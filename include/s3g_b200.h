@@ -268,6 +268,61 @@ int s3g_rasterize_backward_aux(
     const float* dL_dpix_aux,
     float* dL_dcolor_aux);
 
+/* ---- static / dynamic decomposition in one pass (FORWARD ONLY) -------------------------------
+ * render(return_decomposition=True) (gaussian_renderer/__init__.py:177-192) composites the full image, the image of
+ * the dynamic Gaussians alone and that of the static ones alone, and the reference runs its whole rasterizer once per
+ * image.  This entry point does one preprocess, one sort and one composite walk with three accumulator sets.
+ * `group` is a DEVICE uint8 [P] (nonzero = dynamic; may be NULL only when P == 0).  out_color / out_depth / radii
+ * are exactly those of s3g_rasterize_forward on all P Gaussians; out_color_d / out_depth_d and out_color_s /
+ * out_depth_s ([3,H,W] / [1,H,W], all four required) equal s3g_rasterize_forward on the dynamic / static subset
+ * alone - a subset with no Gaussians gives zero images, as P == 0 does.
+ * FORWARD ONLY: the state buffers it leaves carry the group in the staged records and must not be passed to any
+ * backward.  Returns num_rendered of the full image. */
+int64_t s3g_rasterize_forward_split(
+    s3g_alloc_fn geom_alloc, void* geom_user,
+    s3g_alloc_fn binning_alloc, void* binning_user,
+    s3g_alloc_fn image_alloc, void* image_user,
+    int P, int D, int M,
+    const float* background,
+    int width, int height,
+    const float* means3D,
+    const float* shs,
+    const float* colors_precomp,
+    const float* opacities,
+    const float* scales,
+    float scale_modifier,
+    const float* rotations,
+    const float* cov3D_precomp,
+    const float* viewmatrix,
+    const float* projmatrix,
+    const float* cam_pos,
+    float tan_fovx, float tan_fovy,
+    int prefiltered,
+    float* out_color,
+    float* out_depth,
+    int* radii,
+    int debug,
+    void* stream,
+    const uint8_t* group,
+    float* out_color_d,
+    float* out_depth_d,
+    float* out_color_s,
+    float* out_depth_s);
+
+/* ---- evaluation metrics (utils/video_utils.py:210-241 do them in torch and, for SSIM, on the host) ------------
+ * One pass over an image pair, image / gt: DEVICE float [C,H,W] (1 <= C <= 4, H >= 7, W >= 7); mask: DEVICE uint8
+ * [H,W] (nonzero = in) or NULL.  Writes, without host synchronisation, DEVICE double out[4*C+1]:
+ *   out[4c+0] sum of squared errors of channel c        out[4c+1] sum of the SSIM map over the interior
+ *   out[4c+2] the same squared errors summed over mask  out[4c+3] the SSIM map summed over the mask
+ *   out[4C]   number of mask pixels (masked sums are 0 without a mask).
+ * The SSIM map is skimage.metrics.structural_similarity's (>= 0.19, data_range 1, float32 input): 7x7 uniform window
+ * with 'reflect' borders, K1 = 0.01, K2 = 0.03, sample covariances (x 49/48).  "Interior" is the map cropped by 3
+ * pixels on every side (skimage's mean SSIM); the masked sum uses the uncropped map (full=True).
+ * workspace: s3g_eval_metrics_workspace_bytes(C, H, W) bytes. */
+size_t s3g_eval_metrics_workspace_bytes(int C, int H, int W);
+int s3g_eval_metrics(int C, int H, int W, const float* image, const float* gt, const uint8_t* mask,
+                     double* out, void* workspace, void* stream);
+
 /* ---- state-buffer introspection (tests / debugging) ---------------------
  * buffer: 0 = geometry, 1 = binning, 2 = image.  Looks up a named field of our
  * layout for the given problem size and returns its byte offset from the

@@ -37,6 +37,11 @@ SIGNATURES = {
     "s3g_rasterize_backward_aux": (_I, [_I, _I, _I, _I64, _V, _I, _I, _V, _V, _V, _V, _F, _V, _V, _V, _V,
                                         _V, _F, _F, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V,
                                         _V, _V, _V, _I, _V, _V, _V]),
+    "s3g_rasterize_forward_split": (_I64, [ALLOC_FN, _V, ALLOC_FN, _V, ALLOC_FN, _V, _I, _I, _I, _V, _I, _I,
+                                            _V, _V, _V, _V, _V, _F, _V, _V, _V, _V, _V, _F, _F, _I, _V, _V,
+                                            _V, _I, _V, _V, _V, _V, _V, _V]),
+    "s3g_eval_metrics_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "s3g_eval_metrics": (_I, [_I, _I, _I, _V, _V, _V, _V, _V, _V]),
     "s3g_rasterize_backward_dp": (_I, [_I, _I, _I, _I64, _V, _I, _I, _V, _V, _V, _V, _F, _V, _V, _V, _V,
                                        _V, _F, _F, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V,
                                        _V, _V, _V, _I, _V, _V]),

@@ -251,7 +251,9 @@ int64_t forward_impl(s3g_alloc_fn geom_alloc, void* geom_user, s3g_alloc_fn binn
                               const float* viewmatrix, const float* projmatrix, const float* cam_pos,
                               float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
                               float* out_depth, int* radii, int debug, void* stream_,
-                              const float* colors_aux, float* out_aux) {
+                              const float* colors_aux, float* out_aux, const uint8_t* group = nullptr,
+                              float* out_color_d = nullptr, float* out_depth_d = nullptr,
+                              float* out_color_s = nullptr, float* out_depth_s = nullptr) {
     (void)prefiltered;   // the reference only uses it for a device-side trap (auxiliary.h:156-160)
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     if (P < 0 || width <= 0 || height <= 0) return fail(S3G_ERR_ARG, "forward: bad sizes");
@@ -260,7 +262,15 @@ int64_t forward_impl(s3g_alloc_fn geom_alloc, void* geom_user, s3g_alloc_fn binn
     const size_t HW = (size_t)width * height;
     if ((colors_aux != nullptr) != (out_aux != nullptr))
         return fail(S3G_ERR_ARG, "forward: colors_aux and out_color_aux go together");
+    const bool split = out_color_d != nullptr;
+    if (split && colors_aux) return fail(S3G_ERR_ARG, "forward: the split and aux forwards do not combine");
     if (P == 0) {   // rasterize_points.cu:82: outputs stay zero-filled
+        if (split) {
+            S3G_CUDA(cudaMemsetAsync(out_color_d, 0, 3 * HW * sizeof(float), stream), "memset color_d");
+            S3G_CUDA(cudaMemsetAsync(out_depth_d, 0, HW * sizeof(float), stream), "memset depth_d");
+            S3G_CUDA(cudaMemsetAsync(out_color_s, 0, 3 * HW * sizeof(float), stream), "memset color_s");
+            S3G_CUDA(cudaMemsetAsync(out_depth_s, 0, HW * sizeof(float), stream), "memset depth_s");
+        }
         if (out_aux) S3G_CUDA(cudaMemsetAsync(out_aux, 0, 3 * HW * sizeof(float), stream), "memset aux");
         S3G_CUDA(cudaMemsetAsync(out_color, 0, 3 * HW * sizeof(float), stream), "memset color");
         S3G_CUDA(cudaMemsetAsync(out_depth, 0, HW * sizeof(float), stream), "memset depth");
@@ -304,6 +314,9 @@ int64_t forward_impl(s3g_alloc_fn geom_alloc, void* geom_user, s3g_alloc_fn binn
     pa.depth_key = geom.depth_key; pa.tiles_touched = geom.tiles_touched; pa.rect = geom.rect;
     pa.clamped = geom.clamped; pa.order = geom.order_a;
     pa.grid_x = tg.x; pa.grid_y = tg.y;
+    // scan_misc[4]: dynamic-Gaussian count of a split forward (zeroed with the scan state below)
+    pa.group = split ? group : nullptr;
+    pa.group_count = split ? geom.scan_misc + 4 : nullptr;
     g_timer.begin(0);
     // one memset for everything the chained scan and the depth sort expect zeroed (look-back words, tickets,
     // digit histograms)
@@ -424,7 +437,14 @@ int64_t forward_impl(s3g_alloc_fn geom_alloc, void* geom_user, s3g_alloc_fn binn
         ra.final_T = img.final_T; ra.n_contrib = img.n_contrib;
         ra.out_color = out_color; ra.out_depth = out_depth;
         ra.aux = geom.aux; ra.out_aux = out_aux;
-        if (colors_aux) render_forward_kernel<true><<<dim3(tg.x, tg.y), TILE_PIX, 0, stream>>>(ra);
+        if (split) {
+            RenderSplitArgs sa;
+            sa.f = ra;
+            sa.out_color_d = out_color_d; sa.out_depth_d = out_depth_d;
+            sa.out_color_s = out_color_s; sa.out_depth_s = out_depth_s;
+            sa.group_count = geom.scan_misc + 4; sa.P = (uint32_t)P;
+            render_forward_split_kernel<<<dim3(tg.x, tg.y), TILE_PIX, 0, stream>>>(sa);
+        } else if (colors_aux) render_forward_kernel<true><<<dim3(tg.x, tg.y), TILE_PIX, 0, stream>>>(ra);
         else render_forward_kernel<false><<<dim3(tg.x, tg.y), TILE_PIX, 0, stream>>>(ra);
         S3G_STAGE("render_forward");
         S3G_MARK(0, nullptr);
@@ -608,6 +628,27 @@ int64_t s3g_rasterize_forward_aux(s3g_alloc_fn geom_alloc, void* geom_user, s3g_
                         width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations,
                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color,
                         out_depth, radii, debug, stream, colors_aux, out_color_aux);
+}
+
+int64_t s3g_rasterize_forward_split(s3g_alloc_fn geom_alloc, void* geom_user, s3g_alloc_fn binning_alloc,
+                                    void* binning_user, s3g_alloc_fn image_alloc, void* image_user, int P,
+                                    int D, int M, const float* background, int width, int height,
+                                    const float* means3D, const float* shs, const float* colors_precomp,
+                                    const float* opacities, const float* scales, float scale_modifier,
+                                    const float* rotations, const float* cov3D_precomp,
+                                    const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                    float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
+                                    float* out_depth, int* radii, int debug, void* stream,
+                                    const uint8_t* group, float* out_color_d, float* out_depth_d,
+                                    float* out_color_s, float* out_depth_s) {
+    if (!out_color_d || !out_depth_d || !out_color_s || !out_depth_s)
+        return fail(S3G_ERR_ARG, "forward_split: null dynamic/static output");
+    if (P > 0 && !group) return fail(S3G_ERR_ARG, "forward_split: null group");
+    return forward_impl(geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, P, D, M, background,
+                        width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations,
+                        cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color,
+                        out_depth, radii, debug, stream, nullptr, nullptr, group, out_color_d, out_depth_d,
+                        out_color_s, out_depth_s);
 }
 
 int s3g_rasterize_backward(int P, int D, int M, int64_t R, const float* background, int width,

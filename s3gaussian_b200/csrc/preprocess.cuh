@@ -215,6 +215,10 @@ struct PreFwdArgs {
     uint8_t* clamped;
     uint32_t* order;   // identity permutation, input of the depth sort
     int grid_x, grid_y;
+    // static/dynamic split (forward only): group [P] nonzero = dynamic, or NULL.  A dynamic Gaussian gets bit 31 of
+    // its own-index word in Cod.w (P < 2^30 leaves it free); group_count (zeroed) receives the number of them.
+    const uint8_t* group;
+    uint32_t* group_count;
 };
 
 // Conservative per-Gaussian cull threshold used by the tile kernels: a pixel
@@ -364,6 +368,13 @@ __global__ void __launch_bounds__(PRE_THREADS) preprocess_forward_kernel(PreFwdA
         p_orig = {a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2]};
         vis = project_gaussian(a, s_cam, idx, p_orig, po);
     }
+    uint32_t group_bit = 0;
+    if (a.group) {
+        const bool dyn = valid && a.group[idx] != 0;
+        const uint32_t m = __ballot_sync(0xffffffffu, dyn);
+        if (lane == 0 && m) atomicAdd(a.group_count, (uint32_t)__popc(m));
+        group_bit = dyn ? 0x80000000u : 0u;
+    }
 
     float3 col = {0.f, 0.f, 0.f};
     uint8_t clamped = 0;
@@ -388,10 +399,10 @@ __global__ void __launch_bounds__(PRE_THREADS) preprocess_forward_kernel(PreFwdA
     a.depth_key[idx] = __float_as_uint(po.depth);
     a.xyAB[idx] = make_float4(po.pix.x, po.pix.y, po.conic.x, po.conic.y);
     // Cod.w carries the Gaussian's own index: the backward composite takes the target of its REDs from the
-    // staged record instead of a second id table
+    // staged record instead of a second id table (bit 31: the Gaussian's group in a split forward)
     a.Cod[idx] = make_float4(po.conic.z, opacity,
                              cull_tau(opacity, po.conic.x, po.conic.y, po.conic.z, po.lam_max, po.lam_min),
-                             __uint_as_float((uint32_t)idx));
+                             __uint_as_float((uint32_t)idx | group_bit));
     a.rgb[idx] = make_float4(col.x, col.y, col.z, po.depth);
     if (a.colors_aux)
         a.aux[idx] = make_float4(a.colors_aux[3 * idx], a.colors_aux[3 * idx + 1], a.colors_aux[3 * idx + 2], 0.f);

@@ -10,6 +10,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "reduce.cuh"
+
 namespace s3g {
 
 // ---------------------------------------------------------------------------------------------
@@ -130,22 +132,7 @@ constexpr int LOSS_W = LOSS_T + 2 * LOSS_HALO; // 42
 constexpr int LOSS_THREADS = 256;
 
 struct LossWin { float w[11]; };
-
-__device__ __forceinline__ float block_sum_256(float v, float* red) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    __syncthreads();
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    float s = 0.f;
-    if (warp == 0) {
-        s = lane < (LOSS_THREADS / 32) ? red[lane] : 0.f;
-#pragma unroll
-        for (int o = 4; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    }
-    return s;   // valid in thread 0
-}
+static_assert(LOSS_THREADS == 256, "block_sum_256 reduces 256-thread blocks");
 
 // x, y: [planes][H][W] (planes = B*3).  maps: 3 x [planes][H][W].  partial: [blocks][4]
 __global__ void __launch_bounds__(LOSS_THREADS) loss_stats_kernel(int H, int W, const float* __restrict__ x,

@@ -140,6 +140,50 @@ def rasterize_gaussians_aux(means3D, means2D, sh, colors_precomp, opacities, sca
                                      rotations, cov3Ds_precomp, raster_settings, colors_aux)
 
 
+def rasterize_gaussians_split(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                              raster_settings, group):
+    """(color, radii, depth, color_d, depth_d, color_s, depth_s) of s3g_rasterize_forward_split: the full image and
+    the images of the Gaussians with group != 0 (dynamic) and group == 0 (static) alone, from one preprocess, one
+    sort and one composite walk.  Forward only: there is no autograd node."""
+    lib = _lib.load()
+    tensors = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
+    if torch.is_grad_enabled() and any(t.requires_grad for t in tensors + (means2D,)):
+        raise RuntimeError("forward_split has no backward: call it under torch.no_grad() or with detached inputs")
+    if means3D.dim() != 2 or means3D.size(1) != 3:
+        raise RuntimeError("means3D must have dimensions (num_points, 3)")
+    if not means3D.is_cuda:
+        raise RuntimeError("s3gaussian_b200 has no CPU path: means3D must be a CUDA tensor")
+    dev = means3D.device
+    rs = raster_settings
+    P = means3D.size(0)
+    H, W = int(rs.image_height), int(rs.image_width)
+    if group.dtype not in (torch.bool, torch.uint8) or tuple(group.shape) != (P,) or group.device != dev:
+        raise RuntimeError("group must be a bool or uint8 tensor of shape (num_points,) on the Gaussians' device")
+    group = group.contiguous().view(torch.uint8)
+    means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp = (_f32c(t, dev) for t in tensors)
+    bg = _f32c(rs.bg, dev)
+    view = _f32c(rs.viewmatrix, dev)
+    proj = _f32c(rs.projmatrix, dev)
+    campos = _f32c(rs.campos, dev)
+
+    color, color_d, color_s = (torch.empty((3, H, W), dtype=torch.float32, device=dev) for _ in range(3))
+    depth, depth_d, depth_s = (torch.empty((1, H, W), dtype=torch.float32, device=dev) for _ in range(3))
+    radii = torch.empty((P,), dtype=torch.int32, device=dev)
+    lease = _Lease(dev)   # back to the pool on return: later users of the arenas are ordered by the stream
+    geom, binning, img = lease.aset.geom, lease.aset.binning, lease.aset.img
+    M = sh.size(1) if sh.numel() != 0 else 0
+    args = (geom.cb, None, binning.cb, None, img.cb, None, P, int(rs.sh_degree), M, _ptr(bg), W, H,
+            _ptr(means3D), _ptr(sh), _ptr(colors_precomp), _ptr(opacities), _ptr(scales),
+            float(rs.scale_modifier), _ptr(rotations), _ptr(cov3Ds_precomp), _ptr(view),
+            _ptr(proj), _ptr(campos), float(rs.tanfovx), float(rs.tanfovy),
+            int(bool(rs.prefiltered)), color.data_ptr(), depth.data_ptr(), _ptr(radii),
+            int(bool(rs.debug)), _stream_ptr(dev), _ptr(group), color_d.data_ptr(), depth_d.data_ptr(),
+            color_s.data_ptr(), depth_s.data_ptr())
+    with torch.cuda.device(dev):
+        _lib.check(lib.s3g_rasterize_forward_split(*args), "rasterize_gaussians_split")
+    return color, radii, depth, color_d, depth_d, color_s, depth_s
+
+
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
@@ -392,3 +436,22 @@ class GaussianRasterizer(nn.Module):
                                        scales if scales is not None else E, rotations if rotations is not None else E,
                                        cov3D_precomp if cov3D_precomp is not None else E, self.raster_settings,
                                        colors_aux)
+
+    def forward_split(self, means3D, means2D, opacities, group, shs=None, colors_precomp=None, scales=None,
+                      rotations=None, cov3D_precomp=None):
+        """forward() plus the images of the two Gaussian groups alone, from one preprocess + sort + composite:
+        -> (color, radii, depth, color_d, depth_d, color_s, depth_s), where _d / _s are what forward() returns for
+        the Gaussians with group != 0 / group == 0 only.  `group`: bool or uint8 [P] on the device.  Forward only
+        (no autograd node): raises if autograd would record through the inputs.  Not in the reference (its
+        render(return_decomposition=True) calls forward() three times, gaussian_renderer/__init__.py:177-192)."""
+        if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
+            raise Exception('Please provide excatly one of either SHs or precomputed colors!')
+        if ((scales is None or rotations is None) and cov3D_precomp is None) or \
+                ((scales is not None or rotations is not None) and cov3D_precomp is not None):
+            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
+        E = torch.Tensor([])
+        return rasterize_gaussians_split(means3D, means2D, shs if shs is not None else E,
+                                         colors_precomp if colors_precomp is not None else E, opacities,
+                                         scales if scales is not None else E, rotations if rotations is not None else E,
+                                         cov3D_precomp if cov3D_precomp is not None else E, self.raster_settings,
+                                         group)

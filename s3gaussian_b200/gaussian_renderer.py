@@ -153,7 +153,16 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
 
     want_feat = render_feat and "fine" in stage and feat is not None
     rendered_image2 = None
-    if want_feat and hasattr(rasterizer, "forward_aux") and pipe_shared_binning(pipe):
+    # Without autograd (evaluation, utils/video_utils.py:169) the decomposition's full, dynamic and static images come
+    # from one rasterizer pass; with grad enabled the three differentiable passes below stay the only path.
+    split = return_decomposition and dx is not None and not torch.is_grad_enabled()
+    if split:
+        max_values = torch.max(torch.abs(dx), dim=1)[0]
+        dynamic_mask = max_values > torch.mean(max_values)
+        (rendered_image, radii, depth, rendered_image_d, depth_d, rendered_image_s, depth_s) = rasterizer.forward_split(
+            means3D=means3D_final, means2D=means2D, opacities=opacity, group=dynamic_mask, shs=shs_final,
+            colors_precomp=colors_precomp, scales=scales_final, rotations=rotations_final, cov3D_precomp=cov3D_precomp)
+    elif want_feat and hasattr(rasterizer, "forward_aux") and pipe_shared_binning(pipe):
         # the feature image shares preprocess, sort and the per-pixel alpha evaluation with the colour image
         # (the reference rasterizes the same geometry a second time, gaussian_renderer/__init__.py:173-186)
         rendered_image, radii, depth, rendered_image2 = rasterizer.forward_aux(
@@ -174,7 +183,11 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
                 scales=scales_final, rotations=rotations_final, cov3D_precomp=cov3D_precomp)
         result_dict.update({"feat": rendered_image2})
 
-    if return_decomposition and dx is not None:
+    if split:
+        visible = radii > 0
+        result_dict.update({"render_d": rendered_image_d, "depth_d": depth_d, "visibility_filter_d": visible[dynamic_mask],
+                            "render_s": rendered_image_s, "depth_s": depth_s, "visibility_filter_s": visible[~dynamic_mask]})
+    elif return_decomposition and dx is not None:
         max_values = torch.max(torch.abs(dx), dim=1)[0]
         dynamic_mask = max_values > torch.mean(max_values)
         cols = colors_precomp if colors_precomp is not None else None
