@@ -383,6 +383,46 @@ size_t s3g_flow_colors_workspace_bytes(int P);
 int s3g_flow_colors(int P, const float* dx_to, const float* dx_from, int normalize, float* out, void* workspace,
                     void* stream);
 
+/* ---- LPIPS v0.1, AlexNet backbone (utils/video_utils.py:221 calls lpips(rgb, gt_rgb, net_type='alex')) ----------
+ * Restates lpipsPyTorch (csrc/lpips.cuh):
+ *   lpipsPyTorch/__init__.py:19-21          lpips(): LPIPS('alex', '0.1') on x's device, criterion(x, y)
+ *   lpipsPyTorch/modules/networks.py:50-51   z = (x - shift) / scale, shift = [-.030, -.088, -.188],
+ *                                            scale = [.458, .448, .450] (true division; the input is used as given)
+ *   lpipsPyTorch/modules/networks.py:53-63,77-83
+ *                                            torchvision alexnet().features up to the fifth ReLU, taps after the ReLUs
+ *                                            of conv 3->64 11x11/4 pad 2, conv 64->192 5x5 pad 2 (each followed by a
+ *                                            3/2 max-pool, no padding, floor), conv 192->384, 384->256, 256->256 3x3
+ *                                            pad 1; zero padding applies to the z-scored tensor
+ *   lpipsPyTorch/modules/utils.py:6-8        n = f / (sqrt(sum_c f^2) + 1e-10) at each tap
+ *   lpipsPyTorch/modules/lpips.py:30-34      d_l = mean over layer l's grid of sum_c lin_l[c] (n_x - n_y)^2
+ *   lpipsPyTorch/modules/lpips.py:36         sum over the layers and the batch: for N > 1 images, the batch sum
+ * The convolutions are implicit GEMMs on the tensor cores in 3xTF32 with fp32 accumulation; taps, normalisation and
+ * lin weights in fp32; the means and their sum in double.
+ *
+ * s3g_lpips_alex_prepare: once per model, puts the convolution weights into the kernels' K order as tf32 hi/lo tiles
+ * and copies the biases and lin weights, all into `prepared` (DEVICE, s3g_lpips_alex_prepared_bytes(), 16-byte
+ * aligned).  The weights stay the caller's; `prepared` alone is read by s3g_lpips_alex.
+ *
+ * s3g_lpips_alex: x, y DEVICE float [N,3,H,W] (contiguous), N >= 1, H, W >= 31 (smaller sides make the second
+ * max-pool's output empty; torch raises).  Writes, without host synchronisation, DEVICE double out[6]: out[l] the
+ * term of layer l (0..4) summed over the N images, out[5] = out[0] + ... + out[4], the value of lpips(x, y).
+ * Deterministic: no atomics, two calls give bitwise equal results.
+ * workspace: s3g_lpips_alex_workspace_bytes(N, H, W) bytes (0 for invalid sizes).  It holds, for the 2N images (x's,
+ * then y's), every convolution's ReLU output and the two max-pool outputs, channels-last float32, plus the taps'
+ * per-block partial sums: about 0.24 GB for one 1920x1280 pair.
+ * S3G_ERR_ARG before any launch: N < 1, a side below 31, a null pointer, or sizes whose element indices do not fit
+ * 32 bits. */
+typedef struct s3g_lpips_alex_weights {
+    const float* conv_w[5];   /* features.{0,3,6,8,10}.weight, [Cout,Cin,k,k] */
+    const float* conv_b[5];   /* features.{0,3,6,8,10}.bias, [Cout] */
+    const float* lin_w[5];    /* lin{i}.model.1.weight, [1,C,1,1] (C floats) */
+} s3g_lpips_alex_weights;
+size_t s3g_lpips_alex_prepared_bytes(void);
+int s3g_lpips_alex_prepare(const s3g_lpips_alex_weights* weights, void* prepared, void* stream);
+size_t s3g_lpips_alex_workspace_bytes(int N, int H, int W);
+int s3g_lpips_alex(int N, int H, int W, const float* x, const float* y, const void* prepared, double* out,
+                   void* workspace, void* stream);
+
 /* ---- state-buffer introspection (tests / debugging) ---------------------
  * buffer: 0 = geometry, 1 = binning, 2 = image.  Looks up a named field of our
  * layout for the given problem size and returns its byte offset from the

@@ -47,6 +47,11 @@ SIGNATURES = {
     "s3g_flow_colors": (_I, [_I, _V, _V, _I, _V, _V, _V]),
     "s3g_eval_metrics_workspace_bytes": (_SZ, [_I, _I, _I]),
     "s3g_eval_metrics": (_I, [_I, _I, _I, _V, _V, _V, _V, _V, _V]),
+    # s3g_lpips_alex_prepare takes an LpipsAlexWeights (below) with ctypes.byref()
+    "s3g_lpips_alex_prepared_bytes": (_SZ, []),
+    "s3g_lpips_alex_prepare": (_I, [_V, _V, _V]),
+    "s3g_lpips_alex_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "s3g_lpips_alex": (_I, [_I, _I, _I, _V, _V, _V, _V, _V, _V]),
     "s3g_rasterize_backward_dp": (_I, [_I, _I, _I, _I64, _V, _I, _I, _V, _V, _V, _V, _F, _V, _V, _V, _V,
                                        _V, _F, _F, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V,
                                        _V, _V, _V, _I, _V, _V]),
@@ -162,3 +167,8 @@ class PlaneDesc(C.Structure):
 class RowTensor(C.Structure):
     """s3g_row_tensor (include/s3g_b200.h)."""
     _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("row_floats", C.c_int), ("zero_new", C.c_int)]
+
+
+class LpipsAlexWeights(C.Structure):
+    """s3g_lpips_alex_weights (include/s3g_b200.h)."""
+    _fields_ = [("conv_w", C.c_void_p * 5), ("conv_b", C.c_void_p * 5), ("lin_w", C.c_void_p * 5)]

@@ -1,0 +1,188 @@
+// api_lpips.cu - extern "C" entry points of LPIPS (AlexNet, v0.1) (include/s3g_b200.h, csrc/lpips.cuh).
+#include <algorithm>
+#include <cstdint>
+
+#include "api_common.cuh"
+#include "common.cuh"
+#include "lpips.cuh"
+
+using namespace s3g;
+
+namespace {
+inline int fail(int code, const char* what, cudaError_t e = cudaSuccess) { return s3g::api_fail(code, what, e); }
+
+// float offsets inside the prepared buffer: the five layers' weight tiles, then every bias, then every lin weight
+struct LpPrepared {
+    size_t tiles[LP_LAYERS], bias[LP_LAYERS], lin[LP_LAYERS], total;
+    LpPrepared() {
+        size_t o = 0;
+        for (int l = 0; l < LP_LAYERS; ++l) { tiles[l] = o; o += (size_t)lp_tiles(l) * LP_TILE_FLOATS; }
+        for (int l = 0; l < LP_LAYERS; ++l) { bias[l] = o; o += lp_cout(l); }
+        for (int l = 0; l < LP_LAYERS; ++l) { lin[l] = o; o += lp_cout(l); }
+        total = o;
+    }
+};
+
+// the activations of one call: conv output l (channels-last, 2N images), max-pools after conv 1 and 2, tap partials
+struct LpShapes {
+    int64_t h[LP_LAYERS], w[LP_LAYERS];   // conv output sizes (the tap grids)
+    int64_t ph[2], pw[2];                  // max-pool output sizes
+    int64_t conv_elems[LP_LAYERS], pool_elems[2];
+    int64_t tap_blocks[LP_LAYERS];
+    size_t conv_off[LP_LAYERS], pool_off[2], part_off[LP_LAYERS], bytes;
+    LpShapes(int N, int H, int W) {
+        const int64_t NI = 2 * (int64_t)N;
+        int64_t ih = H, iw = W;
+        size_t o = 0;
+        auto take = [&](int64_t bytes_) { const size_t at = o; o += ((size_t)bytes_ + 255) & ~(size_t)255; return at; };
+        for (int l = 0; l < LP_LAYERS; ++l) {
+            h[l] = (ih + 2 * lp_pad(l) - lp_ks(l)) / lp_stride(l) + 1;
+            w[l] = (iw + 2 * lp_pad(l) - lp_ks(l)) / lp_stride(l) + 1;
+            conv_elems[l] = NI * h[l] * w[l] * lp_cout(l);
+            conv_off[l] = take(conv_elems[l] * 4);
+            ih = h[l]; iw = w[l];
+            if (l < 2) {
+                ph[l] = (ih - 3) / 2 + 1; pw[l] = (iw - 3) / 2 + 1;
+                pool_elems[l] = NI * ph[l] * pw[l] * lp_cout(l);
+                pool_off[l] = take(pool_elems[l] * 4);
+                ih = ph[l]; iw = pw[l];
+            }
+        }
+        for (int l = 0; l < LP_LAYERS; ++l) {
+            tap_blocks[l] = div_up64((int64_t)N * h[l] * w[l], LP_TAP_WARPS * LP_TAP_PIX);
+            part_off[l] = take(tap_blocks[l] * 8);
+        }
+        bytes = o + 256;   // + alignment of the base
+    }
+    bool fits_int32() const {
+        for (int l = 0; l < LP_LAYERS; ++l) if (conv_elems[l] >= INT32_MAX) return false;
+        return true;   // the pools are smaller than the convolutions they follow
+    }
+};
+
+bool args_ok(int N, int H, int W) {
+    return N >= 1 && H >= 31 && W >= 31 && (int64_t)N * 3 * H * W < INT32_MAX && LpShapes(N, H, W).fits_int32();
+}
+
+template <int L>
+int launch_conv(const LpConvArgs& a, cudaStream_t stream) {
+    S3G_CUDA(cudaFuncSetAttribute(lpips_conv_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, LP_SMEM_BYTES),
+             "lpips conv smem attribute");
+    const dim3 grid((unsigned)div_up64(a.M, LP_BM), lp_cout(L) / LP_BN);
+    lpips_conv_kernel<L><<<grid, LP_THREADS, LP_SMEM_BYTES, stream>>>(a);
+    S3G_CUDA(cudaGetLastError(), "lpips conv launch");
+    return S3G_OK;
+}
+
+template <int C>
+int launch_tap(int P, int64_t blocks, const float* f, const float* lin, double* partial, cudaStream_t stream) {
+    lpips_tap_kernel<C><<<(unsigned)blocks, 32 * LP_TAP_WARPS, 0, stream>>>(P, f, lin, partial);
+    S3G_CUDA(cudaGetLastError(), "lpips tap launch");
+    return S3G_OK;
+}
+}  // namespace
+
+extern "C" {
+
+size_t s3g_lpips_alex_prepared_bytes(void) { return LpPrepared().total * sizeof(float); }
+
+int s3g_lpips_alex_prepare(const s3g_lpips_alex_weights* wts, void* prepared, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (!wts || !prepared) return fail(S3G_ERR_ARG, "lpips_alex_prepare: null weights/prepared");
+    for (int l = 0; l < LP_LAYERS; ++l)
+        if (!wts->conv_w[l] || !wts->conv_b[l] || !wts->lin_w[l])
+            return fail(S3G_ERR_ARG, "lpips_alex_prepare: null weight pointer");
+    if ((reinterpret_cast<uintptr_t>(prepared) & 15) != 0)
+        return fail(S3G_ERR_ARG, "lpips_alex_prepare: prepared must be 16-byte aligned");
+    const LpPrepared lay;
+    float* dst = static_cast<float*>(prepared);
+    LpPrepArgs p;
+    for (int l = 0; l < LP_LAYERS; ++l) {
+        p.w[l] = wts->conv_w[l];
+        p.dst[l] = dst + lay.tiles[l];
+        S3G_CUDA(cudaMemcpyAsync(dst + lay.bias[l], wts->conv_b[l], lp_cout(l) * sizeof(float), cudaMemcpyDeviceToDevice,
+                                 stream), "lpips_alex_prepare bias copy");
+        S3G_CUDA(cudaMemcpyAsync(dst + lay.lin[l], wts->lin_w[l], lp_cout(l) * sizeof(float), cudaMemcpyDeviceToDevice,
+                                 stream), "lpips_alex_prepare lin copy");
+    }
+    lpips_prep_kernel<<<dim3(256, LP_LAYERS), 256, 0, stream>>>(p);
+    S3G_CUDA(cudaGetLastError(), "lpips_prep launch");
+    return S3G_OK;
+}
+
+size_t s3g_lpips_alex_workspace_bytes(int N, int H, int W) {
+    if (!args_ok(N, H, W)) return 0;
+    return LpShapes(N, H, W).bytes;
+}
+
+int s3g_lpips_alex(int N, int H, int W, const float* x, const float* y, const void* prepared, double* out,
+                   void* workspace, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (N < 1) return fail(S3G_ERR_ARG, "lpips_alex: N >= 1 images expected");
+    if (H < 31 || W < 31) return fail(S3G_ERR_ARG, "lpips_alex: image sides must be >= 31 (AlexNet's second max-pool)");
+    if (!args_ok(N, H, W)) return fail(S3G_ERR_ARG, "lpips_alex: images too large for 32-bit indices");
+    if (!x || !y || !prepared || !out || !workspace) return fail(S3G_ERR_ARG, "lpips_alex: null x/y/prepared/out/workspace");
+    if ((reinterpret_cast<uintptr_t>(prepared) & 15) != 0) return fail(S3G_ERR_ARG, "lpips_alex: unaligned prepared");
+    const LpShapes s(N, H, W);
+    const LpPrepared lay;
+    const float* wp = static_cast<const float*>(prepared);
+    char* base = reinterpret_cast<char*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+    auto buf = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+
+    // conv l reads the pool after conv 1 and 2, the previous conv after that
+    const float* in = nullptr;
+    int ih = H, iw = W;
+    for (int l = 0; l < LP_LAYERS; ++l) {
+        LpConvArgs a;
+        a.in = in; a.x = x; a.y = y; a.N = N; a.H = ih; a.W = iw;
+        a.Ho = (int)s.h[l]; a.Wo = (int)s.w[l];
+        a.M = 2 * N * a.Ho * a.Wo;
+        a.wprep = wp + lay.tiles[l];
+        a.bias = wp + lay.bias[l];
+        a.out = buf(s.conv_off[l]);
+        int rc = S3G_OK;
+        switch (l) {
+            case 0: rc = launch_conv<0>(a, stream); break;
+            case 1: rc = launch_conv<1>(a, stream); break;
+            case 2: rc = launch_conv<2>(a, stream); break;
+            case 3: rc = launch_conv<3>(a, stream); break;
+            default: rc = launch_conv<4>(a, stream); break;
+        }
+        if (rc != S3G_OK) return rc;
+        in = a.out; ih = a.Ho; iw = a.Wo;
+        if (l < 2) {
+            const int C4 = lp_cout(l) / 4;
+            const int total4 = (int)(s.pool_elems[l] / 4);
+            const int grid = (int)std::min<int64_t>(div_up64(total4, 256), (int64_t)device_sm_count() * 16);
+            float* po = buf(s.pool_off[l]);
+            lpips_maxpool_kernel<<<grid, 256, 0, stream>>>(total4, C4, ih, iw, (int)s.ph[l], (int)s.pw[l],
+                                                           reinterpret_cast<const float4*>(in), reinterpret_cast<float4*>(po));
+            S3G_CUDA(cudaGetLastError(), "lpips maxpool launch");
+            in = po; ih = (int)s.ph[l]; iw = (int)s.pw[l];
+        }
+    }
+    LpReduceArgs r;
+    for (int l = 0; l < LP_LAYERS; ++l) {
+        const int P = (int)(N * s.h[l] * s.w[l]);
+        const float* f = buf(s.conv_off[l]);
+        const float* lin = wp + lay.lin[l];
+        double* part = reinterpret_cast<double*>(base + s.part_off[l]);
+        int rc = S3G_OK;
+        switch (lp_cout(l)) {
+            case 64: rc = launch_tap<64>(P, s.tap_blocks[l], f, lin, part, stream); break;
+            case 192: rc = launch_tap<192>(P, s.tap_blocks[l], f, lin, part, stream); break;
+            case 384: rc = launch_tap<384>(P, s.tap_blocks[l], f, lin, part, stream); break;
+            default: rc = launch_tap<256>(P, s.tap_blocks[l], f, lin, part, stream); break;
+        }
+        if (rc != S3G_OK) return rc;
+        r.partial[l] = part;
+        r.blocks[l] = (int)s.tap_blocks[l];
+        r.pixels[l] = (double)(s.h[l] * s.w[l]);
+    }
+    r.out = out;
+    lpips_reduce_kernel<<<1, 256, 0, stream>>>(r);
+    S3G_CUDA(cudaGetLastError(), "lpips reduce launch");
+    return S3G_OK;
+}
+
+}  // extern "C"

@@ -1,0 +1,328 @@
+// lpips.cuh - LPIPS v0.1 with the AlexNet backbone (lpipsPyTorch/modules/{lpips,networks,utils}.py) on the device.
+//
+// Convolutions are implicit GEMMs on the Hopper warpgroup tensor cores, in the decoder's arithmetic (deform_tc.cuh):
+// 3xTF32 (hi*hi + hi*lo + lo*hi) with fp32 accumulators.
+//   M = output pixels of every image of the call (the N images of x, then the N of y), N = output channels,
+//   K = kh * kw * Cin.  CTA = 128 threads = one warpgroup = a 128-pixel x 64-channel output tile (two M = 64 halves of
+//   wgmma m64n64k8); thread r gathers the im2col row of pixel r.  K runs in chunks of 32: the chunk's A (128 x 32) and
+//   B (64 x 32) hi/lo operands sit in shared memory in the canonical K-major layout (umma.cuh); two stages, so the
+//   gather of chunk c + 1 runs while the wgmmas of chunk c do.  Bias and ReLU are applied in the epilogue.
+//   * Layer 1 reads the caller's [N,3,H,W] images and z-scores them in its gather, (v - shift) / scale with a true
+//     division, so the zero padding lands on the z-scored tensor; its K order is PyTorch's (c, ky, kx), 363 padded
+//     to 384.
+//   * Layers 2-5 read internal channels-last (HWC) activations; K order (ky, kx, c), so a 32-wide chunk is 32
+//     consecutive channels of one input pixel (every Cin is a multiple of 32): eight 16-byte loads, or zeros in the
+//     padding.
+// Weights are prepared once per model (lpips_prep_kernel): each layer becomes [Cout / 64][Kpad / 32] tiles of
+// 64 x 32 canonical hi | lo (tf32 round-to-nearest split), 16 KB each, copied per chunk with cp.async.
+// Max-pool (3/2, no padding, floor) is a channels-last kernel of its own.
+// Taps: one warp per pixel pair normalises both feature vectors over channels, weighs the squared difference with
+// the lin weights and sums it; blocks write double partials, and one fixed-order double reduction writes each
+// layer's mean over its grid (summed over the images) and the total.  No atomics: two calls are bitwise equal.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "umma.cuh"
+
+namespace s3g {
+
+constexpr int LP_LAYERS = 5;
+constexpr int LP_BM = 128, LP_BN = 64, LP_BK = 32;
+constexpr int LP_THREADS = 128;
+constexpr int LP_A_FLOATS = LP_BM * LP_BK;               // one operand part (hi or lo) of A
+constexpr int LP_B_FLOATS = LP_BN * LP_BK;
+constexpr int LP_TILE_FLOATS = 2 * LP_B_FLOATS;          // one prepared weight tile: hi | lo
+constexpr int LP_STAGE_FLOATS = 2 * LP_A_FLOATS + LP_TILE_FLOATS;
+constexpr int LP_SMEM_BYTES = 2 * LP_STAGE_FLOATS * 4;   // 96 KB: two stages, two CTAs per SM
+constexpr int LP_TAP_WARPS = 8, LP_TAP_PIX = 8;          // tap kernel: 8 warps x 8 pixels per block
+
+// AlexNet `features` convolutions 0, 3, 6, 8, 10
+__host__ __device__ constexpr int lp_cin(int l) { return l == 0 ? 3 : l == 1 ? 64 : l == 2 ? 192 : l == 3 ? 384 : 256; }
+__host__ __device__ constexpr int lp_cout(int l) { return l == 0 ? 64 : l == 1 ? 192 : l == 2 ? 384 : 256; }
+__host__ __device__ constexpr int lp_ks(int l) { return l == 0 ? 11 : l == 1 ? 5 : 3; }
+__host__ __device__ constexpr int lp_stride(int l) { return l == 0 ? 4 : 1; }
+__host__ __device__ constexpr int lp_pad(int l) { return l <= 1 ? 2 : 1; }
+
+__host__ __device__ constexpr int lp_k(int l) { return lp_ks(l) * lp_ks(l) * lp_cin(l); }
+__host__ __device__ constexpr int lp_kpad(int l) { return (lp_k(l) + LP_BK - 1) / LP_BK * LP_BK; }
+__host__ __device__ constexpr int lp_tiles(int l) { return (lp_cout(l) / LP_BN) * (lp_kpad(l) / LP_BK); }
+
+// hi = x as is (the tensor core reads its tf32 bits), lo = the truncated remainder (deform.cuh's split_tf32)
+__device__ __forceinline__ void lp_split(float x, uint32_t& hi, uint32_t& lo) {
+    hi = __float_as_uint(x);
+    lo = __float_as_uint(x - __uint_as_float(hi & 0xffffe000u));
+}
+
+// ---- weight preparation ------------------------------------------------------------------------------------------
+struct LpPrepArgs {
+    const float* w[LP_LAYERS];    // [Cout][Cin][k][k], PyTorch layout
+    float* dst[LP_LAYERS];        // lp_tiles(l) prepared tiles
+};
+// blockIdx.y = layer; element (co, k) of the padded [Cout][Kpad] matrix in the kernel's K order
+__global__ void __launch_bounds__(256) lpips_prep_kernel(const __grid_constant__ LpPrepArgs p) {
+    const int l = blockIdx.y;
+    const int Cin = lp_cin(l), KS = lp_ks(l), K = lp_k(l), KP = lp_kpad(l), KC = KP / LP_BK;
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < lp_cout(l) * KP; e += gridDim.x * blockDim.x) {
+        const int co = e / KP, k = e - co * KP;
+        float v = 0.f;
+        if (k < K) {
+            int src = k;                                  // layer 1: (c, ky, kx) is PyTorch's own order
+            if (l > 0) {                                  // (ky, kx, c) -> (c, ky, kx)
+                const int tap = k / Cin, c = k - tap * Cin;
+                src = c * KS * KS + tap;
+            }
+            v = __ldg(p.w[l] + (size_t)co * K + src);
+        }
+        uint32_t hi, lo;
+        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(v));
+        const float r = v - __uint_as_float(hi);
+        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(r));
+        float* t = p.dst[l] + (size_t)((co / LP_BN) * KC + k / LP_BK) * LP_TILE_FLOATS;
+        const int ci = umma::canon_idx(co % LP_BN, k % LP_BK, LP_BK);
+        t[ci] = __uint_as_float(hi);
+        t[LP_B_FLOATS + ci] = __uint_as_float(lo);
+    }
+}
+
+// ---- convolution -------------------------------------------------------------------------------------------------
+struct LpConvArgs {
+    const float* in;        // layers 2-5: [2N][H][W][Cin] channels-last
+    const float* x;         // layer 1: images 0..N-1, [N][3][H][W]
+    const float* y;         // layer 1: images N..2N-1
+    int N;                  // images per input (layer 1)
+    int H, W;               // input size
+    int Ho, Wo;             // output size
+    int M;                  // 2N * Ho * Wo
+    const float* wprep;     // this layer's prepared tiles
+    const float* bias;      // [Cout]
+    float* out;             // [2N][Ho][Wo][Cout] channels-last, ReLU applied
+};
+
+__device__ __forceinline__ void lp_cp16(float* sdst, const float* gsrc) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(umma::smem_u32(sdst)), "l"(gsrc) : "memory");
+}
+
+template <int L>
+__global__ void __launch_bounds__(LP_THREADS, 2) lpips_conv_kernel(const __grid_constant__ LpConvArgs a) {
+    constexpr int Cin = lp_cin(L), Cout = lp_cout(L), KS = lp_ks(L), S = lp_stride(L), PAD = lp_pad(L);
+    constexpr int K = lp_k(L), KC = lp_kpad(L) / LP_BK;
+    constexpr uint32_t SBO = (LP_BK / 4) * 128u, MHALF = 8u * SBO;
+    extern __shared__ __align__(128) float s_lp[];
+    const int tid = threadIdx.x;
+    const int m = blockIdx.x * LP_BM + tid;
+    const bool valid = m < a.M;
+    const int hw = a.Ho * a.Wo;
+    const int img = valid ? m / hw : 0;
+    const int pix = valid ? m - img * hw : 0;
+    const int oy = pix / a.Wo, ox = pix - oy * a.Wo;
+    const int iy0 = oy * S - PAD, ix0 = ox * S - PAD;
+    const float* wtiles = a.wprep + (size_t)blockIdx.y * KC * LP_TILE_FLOATS;
+    const float* src = nullptr;     // layer 1: channel 0 of this pixel's image
+    if constexpr (L == 0) src = (img < a.N ? a.x + (size_t)img * 3 * a.H * a.W : a.y + (size_t)(img - a.N) * 3 * a.H * a.W);
+
+    // this thread's 32 A values of chunk c (zero outside the image, past K and past M)
+    float v[LP_BK];
+    auto gather = [&](int c) {
+        const int k0 = c * LP_BK;
+        if constexpr (L == 0) {
+#pragma unroll
+            for (int j = 0; j < LP_BK; ++j) {
+                const int k = k0 + j;
+                const int ch = k / (KS * KS), t = k - ch * (KS * KS), ky = t / KS, kx = t - ky * KS;
+                const int iy = iy0 + ky, ix = ix0 + kx;
+                // the float32 buffers of networks.py:41-44
+                const float shift = ch == 0 ? -.030f : ch == 1 ? -.088f : -.188f;
+                const float scale = ch == 0 ? .458f : ch == 1 ? .448f : .450f;
+                float z = 0.f;
+                if (valid && k < K && iy >= 0 && iy < a.H && ix >= 0 && ix < a.W)
+                    z = __fdiv_rn(__fsub_rn(__ldg(src + ((size_t)ch * a.H + iy) * a.W + ix), shift), scale);
+                v[j] = z;
+            }
+        } else {
+            const int tap = k0 / Cin, c0 = k0 - tap * Cin, ky = tap / KS, kx = tap - ky * KS;
+            const int iy = iy0 + ky, ix = ix0 + kx;
+            const bool in = valid && iy >= 0 && iy < a.H && ix >= 0 && ix < a.W;
+            const float4* p = reinterpret_cast<const float4*>(a.in + (((size_t)img * a.H + (in ? iy : 0)) * a.W + (in ? ix : 0)) * Cin + c0);
+#pragma unroll
+            for (int j = 0; j < LP_BK / 4; ++j) {
+                const float4 q = in ? __ldg(p + j) : make_float4(0.f, 0.f, 0.f, 0.f);
+                v[4 * j] = q.x; v[4 * j + 1] = q.y; v[4 * j + 2] = q.z; v[4 * j + 3] = q.w;
+            }
+        }
+    };
+    // A values -> hi/lo operand tiles of `stage`; the chunk's weight tile -> the stage's B by cp.async
+    auto stage_in = [&](int c, int stage) {
+        float* st = s_lp + stage * LP_STAGE_FLOATS;
+        const float* wt = wtiles + (size_t)c * LP_TILE_FLOATS;
+#pragma unroll
+        for (int j = 0; j < LP_TILE_FLOATS / 4 / LP_THREADS; ++j)
+            lp_cp16(st + 2 * LP_A_FLOATS + 4 * (tid + j * LP_THREADS), wt + 4 * (tid + j * LP_THREADS));
+        asm volatile("cp.async.commit_group;" ::: "memory");
+#pragma unroll
+        for (int j = 0; j < LP_BK; j += 4) {
+            uint32_t h[4], lo[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) lp_split(v[j + i], h[i], lo[i]);
+            const int ci = umma::canon_idx(tid, j, LP_BK);
+            *reinterpret_cast<uint4*>(st + ci) = make_uint4(h[0], h[1], h[2], h[3]);
+            *reinterpret_cast<uint4*>(st + LP_A_FLOATS + ci) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+        }
+    };
+
+    float acc[2][LP_BN / 2];
+    gather(0);
+    stage_in(0, 0);
+    for (int c = 0; c < KC; ++c) {
+        asm volatile("cp.async.wait_all;" ::: "memory");
+        umma::fence_async_smem();
+        __syncthreads();
+        const float* st = s_lp + (c & 1) * LP_STAGE_FLOATS;
+        const uint32_t a_hi = umma::smem_u32(st), a_lo = a_hi + LP_A_FLOATS * 4u;
+        const uint32_t b_hi = a_hi + 2u * LP_A_FLOATS * 4u, b_lo = b_hi + LP_B_FLOATS * 4u;
+        umma::fence_regs(acc[0]); umma::fence_regs(acc[1]);
+        umma::wgmma_fence();
+#pragma unroll
+        for (int k0 = 0; k0 < LP_BK; k0 += 8) {
+            const uint32_t off = (uint32_t)(k0 / 4) * 128u;
+            const uint64_t dbh = umma::make_smem_desc(b_hi + off, 128, SBO), dbl = umma::make_smem_desc(b_lo + off, 128, SBO);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const uint64_t dah = umma::make_smem_desc(a_hi + h * MHALF + off, 128, SBO);
+                const uint64_t dal = umma::make_smem_desc(a_lo + h * MHALF + off, 128, SBO);
+                umma::wgmma_tf32<LP_BN>(acc[h], dal, dbh, c > 0 || k0 > 0);
+                umma::wgmma_tf32<LP_BN>(acc[h], dah, dbl, true);
+                umma::wgmma_tf32<LP_BN>(acc[h], dah, dbh, true);
+            }
+        }
+        umma::wgmma_commit();
+        // the other stage was last read by chunk c - 1's wgmmas, complete since that iteration's wait
+        if (c + 1 < KC) {
+            gather(c + 1);
+            stage_in(c + 1, (c + 1) & 1);
+        }
+        umma::wgmma_wait_all();
+        umma::fence_regs(acc[0]); umma::fence_regs(acc[1]);
+    }
+    // epilogue: + bias, ReLU, channels-last store (fragment layout, umma.cuh)
+    const int n0 = blockIdx.y * LP_BN;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int i = 0; i < LP_BN / 2; i += 2) {
+            const int row = blockIdx.x * LP_BM + 64 * h + umma::frag_row(i);
+            const int col = n0 + umma::frag_col(i);
+            if (row < a.M) {
+                const float b0 = __ldg(a.bias + col), b1 = __ldg(a.bias + col + 1);
+                *reinterpret_cast<float2*>(a.out + (size_t)row * Cout + col) =
+                    make_float2(fmaxf(acc[h][i] + b0, 0.f), fmaxf(acc[h][i + 1] + b1, 0.f));
+            }
+        }
+    }
+}
+
+// ---- max-pool 3/2, no padding, floor mode, channels-last [NI][H][W][C] -> [NI][Ho][Wo][C] ---------------------------
+__global__ void __launch_bounds__(256) lpips_maxpool_kernel(int total4, int C4, int H, int W, int Ho, int Wo,
+                                                            const float4* __restrict__ in, float4* __restrict__ out) {
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < total4; e += gridDim.x * blockDim.x) {
+        const int c = e % C4;
+        int r = e / C4;
+        const int ox = r % Wo;
+        r /= Wo;
+        const int oy = r % Ho, n = r / Ho;
+        const float4* p = in + (((size_t)n * H + 2 * oy) * W + 2 * ox) * C4 + c;
+        float4 m = __ldg(p);
+#pragma unroll
+        for (int dy = 0; dy < 3; ++dy)
+#pragma unroll
+            for (int dx = 0; dx < 3; ++dx) {
+                const float4 q = __ldg(p + ((size_t)dy * W + dx) * C4);
+                m.x = fmaxf(m.x, q.x); m.y = fmaxf(m.y, q.y); m.z = fmaxf(m.z, q.z); m.w = fmaxf(m.w, q.w);
+            }
+        out[e] = m;
+    }
+}
+
+// ---- taps --------------------------------------------------------------------------------------------------------
+// pixel p < P = N * Hl * Wl of feature map f [2N][Hl][Wl][C]: x's features at row p, y's at row P + p.
+// d(p) = sum_c w_c (fx_c / (|fx| + 1e-10) - fy_c / (|fy| + 1e-10))^2; partial[block] = sum of its pixels' d.
+template <int C>
+__global__ void __launch_bounds__(32 * LP_TAP_WARPS) lpips_tap_kernel(int P, const float* __restrict__ f,
+                                                                       const float* __restrict__ lin,
+                                                                       double* __restrict__ partial) {
+    constexpr int PER = C / 32;
+    __shared__ double s_w[LP_TAP_WARPS];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float w[PER];
+#pragma unroll
+    for (int i = 0; i < PER; ++i) w[i] = __ldg(lin + lane + 32 * i);
+    double wsum = 0.0;
+    for (int j = 0; j < LP_TAP_PIX; ++j) {
+        const int p = (blockIdx.x * LP_TAP_WARPS + warp) * LP_TAP_PIX + j;
+        if (p >= P) break;
+        const float* fx = f + (size_t)p * C;
+        const float* fy = f + ((size_t)P + p) * C;
+        float xv[PER], yv[PER], sx = 0.f, sy = 0.f;
+#pragma unroll
+        for (int i = 0; i < PER; ++i) {
+            xv[i] = __ldg(fx + lane + 32 * i);
+            yv[i] = __ldg(fy + lane + 32 * i);
+            sx = fmaf(xv[i], xv[i], sx);
+            sy = fmaf(yv[i], yv[i], sy);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            sx += __shfl_xor_sync(0xffffffffu, sx, o);
+            sy += __shfl_xor_sync(0xffffffffu, sy, o);
+        }
+        const float nx = sqrtf(sx) + 1e-10f, ny = sqrtf(sy) + 1e-10f;
+        float d = 0.f;
+#pragma unroll
+        for (int i = 0; i < PER; ++i) {
+            const float t = __fdiv_rn(xv[i], nx) - __fdiv_rn(yv[i], ny);
+            d = fmaf(w[i], t * t, d);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+        wsum += (double)d;
+    }
+    if (lane == 0) s_w[warp] = wsum;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+#pragma unroll
+        for (int i = 0; i < LP_TAP_WARPS; ++i) s += s_w[i];
+        partial[blockIdx.x] = s;
+    }
+}
+
+struct LpReduceArgs {
+    const double* partial[LP_LAYERS];
+    int blocks[LP_LAYERS];
+    double pixels[LP_LAYERS];     // Hl * Wl: the layer's mean is over its own grid
+    double* out;                  // [6]
+};
+// one block: out[l] = sum of layer l's partials / pixels[l] in a fixed order, out[5] = out[0] + ... + out[4]
+__global__ void __launch_bounds__(256) lpips_reduce_kernel(const __grid_constant__ LpReduceArgs r) {
+    __shared__ double red[256];
+    double total = 0.0;
+    for (int l = 0; l < LP_LAYERS; ++l) {
+        double s = 0.0;
+        for (int i = threadIdx.x; i < r.blocks[l]; i += 256) s += r.partial[l][i];
+        red[threadIdx.x] = s;
+        __syncthreads();
+        for (int o = 128; o > 0; o >>= 1) {
+            if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+            __syncthreads();
+        }
+        if (threadIdx.x == 0) {
+            const double m = red[0] / r.pixels[l];
+            r.out[l] = m;
+            total += m;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) r.out[LP_LAYERS] = total;
+}
+
+}  // namespace s3g

@@ -158,7 +158,7 @@ def render_pixels(viewpoint_stack, gaussians, bg, pipe, compute_metrics: bool = 
     With the fine stage's dx (not no_dx), also dx_list (the per-view dx, device tensors) and, from four views on,
     forward_flows / backward_flows (lists of HWC numpy arrays in the reference's order, see flow_plan); `debug`
     min-max normalises the flow colours, as the reference's.  lpips is -1 unless `lpips_fn(rgb, gt)` (-> tensor) is
-    given: the reference's LPIPS needs downloaded AlexNet weights.  Not covered: save_seperate_pcd (render_func
+    given; s3gaussian_b200.lpips.LPIPS() computes the reference's LPIPS on the device.  Not covered: save_seperate_pcd (render_func
     :243-249), which render_pixels never enables.
     """
     from .gaussian_renderer import dynamic_mask_of, fine_front, raster_settings_for
