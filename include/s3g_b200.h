@@ -14,9 +14,9 @@
  *                              (pybind: _C.rasterize_gaussians           DGR/ext.cpp:16, DGR/rasterize_points.cu:35-117)
  *   s3g_rasterize_backward  <- CudaRasterizer::Rasterizer::backward      DGR/cuda_rasterizer/rasterizer.h:58-88
  *                              (pybind: _C.rasterize_gaussians_backward  DGR/ext.cpp:17, DGR/rasterize_points.cu:119-202)
- *   s3g_deform_forward /    <- deform_network.forward_dynamic            scene/deformation.py:216-231
- *   s3g_deform_backward        + HexPlaneField.forward                   scene/hexplane.py:160-183
- *                              + activations / Python SH->RGB            gaussian_renderer/__init__.py:99-117
+ *   s3g_deform_forward_save /  <- deform_network.forward_dynamic         scene/deformation.py:216-231
+ *   s3g_deform_backward_saved     + HexPlaneField.forward                scene/hexplane.py:160-183
+ *                                 + activations / Python SH->RGB         gaussian_renderer/__init__.py:99-117
  *
  * Conventions (identical to the reference):
  *   - all pointers are DEVICE pointers unless the name says host;
@@ -452,21 +452,12 @@ typedef struct s3g_deform_net_grads {
  * colors [P,3] = clamp_min(SH(shs+dshs, dir(xyz - campos)) + 0.5, 0) with the UNDEFORMED xyz,
  * dx [P,3], dshs [P,16,3], feat [P,3].  Pointers of disabled heads may be NULL.
  * features [P, 32*num_levels] receives the sampled HexPlane features (the hand-over between the
- * sampling and the decoder kernel); keep it for s3g_deform_backward.
- * campos: device float[3]; sh_degree: active degree (0..3). */
-int s3g_deform_forward(const s3g_deform_net* net, int P, const float* xyz, const float* scales,
-                       const float* rotations, const float* opacity, const float* shs, float time,
-                       const float* campos, int sh_degree,
-                       float* means3D, float* scales_act, float* rot_act, float* opacity_act,
-                       float* colors, float* dx, float* dshs, float* feat, float* features,
-                       void* workspace, void* stream);
-/* bytes of `workspace` for s3g_deform_forward (tensor-core-ready copies of the Linear weights) */
-size_t s3g_deform_forward_workspace_bytes(const s3g_deform_net* net);
-
-/* Training variant: the same forward, which also keeps the decoder's hidden activations (h = feature_out(f) and the
- * hidden layer of every enabled head, scene/deformation.py:56-76 - what autograd keeps for the reference) in the
- * opaque buffer `acts` of s3g_deform_saved_bytes(net, P) bytes, so that s3g_deform_backward_saved does not
- * recompute them.  acts == NULL: identical to s3g_deform_forward.  (1 <= num_levels <= 4; feat_dim 32; width 64.) */
+ * sampling and the decoder kernel); keep it for s3g_deform_backward_saved.
+ * acts receives the decoder's hidden activations (h = feature_out(f) and the hidden layer of every enabled head,
+ * scene/deformation.py:56-76 - what autograd keeps for the reference): an opaque buffer of
+ * s3g_deform_saved_bytes(net, P) bytes that s3g_deform_backward_saved reads.  acts may be NULL when no backward
+ * will follow.
+ * campos: device float[3]; sh_degree: active degree (0..3).  (1 <= num_levels <= 4; feat_dim 32; width 64.) */
 size_t s3g_deform_saved_bytes(const s3g_deform_net* net, int P);
 int s3g_deform_forward_save(const s3g_deform_net* net, int P, const float* xyz, const float* scales,
                             const float* rotations, const float* opacity, const float* shs, float time,
@@ -474,21 +465,14 @@ int s3g_deform_forward_save(const s3g_deform_net* net, int P, const float* xyz, 
                             float* means3D, float* scales_act, float* rot_act, float* opacity_act,
                             float* colors, float* dx, float* dshs, float* feat, float* features, float* acts,
                             void* workspace, void* stream);
+/* bytes of `workspace` for s3g_deform_forward_save (tensor-core-ready copies of the Linear weights) */
+size_t s3g_deform_forward_workspace_bytes(const s3g_deform_net* net);
 
 /* Backward of the above.  g_* are dL/d(output) (NULL = zero).  Writes dL/d(raw inputs)
  * [P,*] in full, overwrites the Linear gradients in `grads` and accumulates the plane
- * gradients.  `features` is the buffer the forward filled.  `workspace` must hold
- * s3g_deform_workspace_bytes(net, P) bytes. */
+ * gradients.  `features` and `acts` are the buffers the forward filled; acts is required for P > 0.
+ * `workspace` must hold s3g_deform_workspace_bytes(net, P) bytes. */
 size_t s3g_deform_workspace_bytes(const s3g_deform_net* net, int P);
-int s3g_deform_backward(const s3g_deform_net* net, int P, const float* xyz, const float* scales,
-                        const float* rotations, const float* opacity, const float* shs, float time,
-                        const float* campos, int sh_degree, const float* features,
-                        const float* g_means3D, const float* g_scales_act, const float* g_rot_act,
-                        const float* g_opacity_act, const float* g_colors, const float* g_dx,
-                        const float* g_dshs, const float* g_feat,
-                        float* d_xyz, float* d_scales, float* d_rotations, float* d_opacity, float* d_shs,
-                        const s3g_deform_net_grads* grads, void* workspace, void* stream);
-/* Same with the hidden activations s3g_deform_forward_save stored (acts == NULL: recompute, as above). */
 int s3g_deform_backward_saved(const s3g_deform_net* net, int P, const float* xyz, const float* scales,
                               const float* rotations, const float* opacity, const float* shs, float time,
                               const float* campos, int sh_degree, const float* features, const float* acts,

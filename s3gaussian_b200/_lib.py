@@ -56,13 +56,11 @@ SIGNATURES = {
     "s3g_state_field": (_I, [_I, C.c_char_p, _I64, _I64, _I, _I, C.POINTER(_SZ), C.POINTER(_SZ),
                              C.POINTER(_SZ)]),
     # struct pointers (s3g_deform_net / s3g_deform_net_grads) are passed with ctypes.byref()
-    "s3g_deform_forward": (_I, [_V, _I] + [_V] * 5 + [_F, _V, _I] + [_V] * 9 + [_V, _V]),
     "s3g_deform_forward_workspace_bytes": (_SZ, [_V]),
     "s3g_deform_saved_bytes": (_SZ, [_V, _I]),
     "s3g_deform_forward_save": (_I, [_V, _I] + [_V] * 5 + [_F, _V, _I] + [_V] * 9 + [_V] + [_V, _V]),
     "s3g_deform_backward_saved": (_I, [_V, _I] + [_V] * 5 + [_F, _V, _I] + [_V, _V] + [_V] * 8 + [_V] * 5 + [_V, _V, _V]),
     "s3g_deform_workspace_bytes": (_SZ, [_V, _I]),
-    "s3g_deform_backward": (_I, [_V, _I] + [_V] * 5 + [_F, _V, _I] + [_V] + [_V] * 8 + [_V] * 5 + [_V, _V, _V]),
     "s3g_umma_selftest": (_I, [_V, _V, _V, _I, _I, _I, _V]),
     "s3g_profile_enable": (_I, [_I]),
     "s3g_profile_read": (_I, [_I, _V, _I]),

@@ -39,15 +39,6 @@ int deform_grid(int ntiles, int ctas_per_sm = 1) {
 
 extern "C" {
 
-int s3g_deform_forward(const s3g_deform_net* net, int P, const float* xyz, const float* scales,
-                       const float* rotations, const float* opacity, const float* shs, float time,
-                       const float* campos, int sh_degree, float* means3D, float* scales_act,
-                       float* rot_act, float* opacity_act, float* colors, float* dx, float* dshs,
-                       float* feat, float* features, void* workspace, void* stream_) {
-    return s3g_deform_forward_save(net, P, xyz, scales, rotations, opacity, shs, time, campos, sh_degree, means3D, scales_act,
-                                   rot_act, opacity_act, colors, dx, dshs, feat, features, nullptr, workspace, stream_);
-}
-
 int s3g_deform_forward_save(const s3g_deform_net* net, int P, const float* xyz, const float* scales,
                             const float* rotations, const float* opacity, const float* shs, float time,
                             const float* campos, int sh_degree, float* means3D, float* scales_act,

@@ -57,18 +57,6 @@ size_t s3g_deform_workspace_bytes(const s3g_deform_net* net, int P) {
            tacc_floats(d) * sizeof(float) + 256;
 }
 
-int s3g_deform_backward(const s3g_deform_net* net, int P, const float* xyz, const float* scales,
-                        const float* rotations, const float* opacity, const float* shs, float time,
-                        const float* campos, int sh_degree, const float* features,
-                        const float* g_means3D, const float* g_scales_act, const float* g_rot_act, const float* g_opacity_act,
-                        const float* g_colors, const float* g_dx, const float* g_dshs, const float* g_feat,
-                        float* d_xyz, float* d_scales, float* d_rotations, float* d_opacity, float* d_shs,
-                        const s3g_deform_net_grads* grads, void* workspace, void* stream_) {
-    return s3g_deform_backward_saved(net, P, xyz, scales, rotations, opacity, shs, time, campos, sh_degree, features, nullptr,
-                                     g_means3D, g_scales_act, g_rot_act, g_opacity_act, g_colors, g_dx, g_dshs, g_feat,
-                                     d_xyz, d_scales, d_rotations, d_opacity, d_shs, grads, workspace, stream_);
-}
-
 int s3g_deform_backward_saved(const s3g_deform_net* net, int P, const float* xyz, const float* scales,
                               const float* rotations, const float* opacity, const float* shs, float time,
                               const float* campos, int sh_degree, const float* features, const float* acts,
@@ -84,6 +72,8 @@ int s3g_deform_backward_saved(const s3g_deform_net* net, int P, const float* xyz
     if (!grads || !workspace) return fail(S3G_ERR_ARG, "deform_backward: null grads/workspace");
     if (P > 0 && (!xyz || !scales || !rotations || !opacity || !shs || !campos || !features))
         return fail(S3G_ERR_ARG, "deform_backward: null input");
+    if (P > 0 && !acts)
+        return fail(S3G_ERR_ARG, "deform_backward: null acts (the hidden activations s3g_deform_forward_save keeps)");
     if (P > 0 && (!d_xyz || !d_scales || !d_rotations || !d_opacity || !d_shs))
         return fail(S3G_ERR_ARG, "deform_backward: null output");
     if (sh_degree < 0 || sh_degree > 3) return fail(S3G_ERR_ARG, "deform_backward: sh_degree must be 0..3");
@@ -99,12 +89,10 @@ int s3g_deform_backward_saved(const s3g_deform_net* net, int P, const float* xyz
             if (!a.gplanes[l][k]) return fail(S3G_ERR_ARG, "deform_backward: null plane gradient");
         }
     make_offsets(d, a.off);
-    const bool saved = acts != nullptr && act_slots(d, a.act_slot) > 0;
-    if (acts && !saved) return fail(S3G_ERR_ARG, "deform_backward: this net's forward stores no activations (s3g_deform_saved_bytes == 0)");
-    if (!saved) act_slots(d, a.act_slot);
-    a.acts = saved ? acts : nullptr;
+    act_slots(d, a.act_slot);
+    a.acts = acts;
     a.act_stride = (size_t)((P + 127) / 128) * 128 * 64;
-    build_wseq(d, true, a.wseq, saved);
+    build_wseq(d, a.wseq);
     a.partial = reinterpret_cast<float*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
     a.features = features;
     a.dfeatures = a.partial + (size_t)kMaxBwdGrid * a.off.total;
@@ -141,8 +129,7 @@ int s3g_deform_backward_saved(const s3g_deform_net* net, int P, const float* xyz
             kernel<<<grid, DTHREADS, smem, stream>>>(a);
             return S3G_OK;
         };
-        if (saved) rc = d.L == 4 ? launch(deform_backward_kernel<4, true>) : launch(deform_backward_kernel<0, true>);
-        else rc = d.L == 4 ? launch(deform_backward_kernel<4, false>) : launch(deform_backward_kernel<0, false>);
+        rc = d.L == 4 ? launch(deform_backward_kernel<4>) : launch(deform_backward_kernel<0>);
         if (rc != S3G_OK) return rc;
         S3G_CUDA(cudaGetLastError(), "deform_backward launch");
         ScatterArgs sc;

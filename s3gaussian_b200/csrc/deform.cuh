@@ -13,7 +13,7 @@
 //                                         plain TF32 / BF16, ~1e-3), xyz+dx, exp / normalize / sigmoid, SH->RGB with
 //                                         the undeformed view direction fused into the epilogues
 //   backward  deform_backward_kernel      mma.sync 3xTF32, tiles of 64 Gaussians: the hidden activations come from
-//                                         what the wgmma forward kept (SAVED) or are recomputed from the features;
+//                                         what the wgmma forward kept;
 //                                         push-back through the heads, Linear gradients into per-CTA partial buffers
 //                                         (deform_reduce_kernel sums them), dL/d(features) [P][32L]
 //             hexplane_scatter_kernel     plane gradients with 128-bit REDs (time planes: per-texel sums +
@@ -163,10 +163,10 @@ struct WPipe {
     __device__ __forceinline__ void release() const { asm volatile("cp.async.wait_all;" ::: "memory"); }
 };
 
-// out[g][n] = act_out( sum_k act_in(in[g][k]) * W[n][k] + b[n] ),  g < 64, n < N (N = 64 or 48).
+// out[g][n] = sum_k in[g][k] * W[n][k] + b[n],  g < 64, n < N (N = 64 or 48).
 // 16 warps: (warp & 3) picks 16 rows, (warp >> 2) picks 16 of the columns (N = 48: the last group idles).
 // sIn / sOut / sW are distinct smem regions; ends with a __syncthreads().
-template <int K, int N, bool RELU_IN, bool RELU_OUT>
+template <int K, int N>
 __device__ __forceinline__ void tile_linear(const float* sIn, int inStride, WPipe& pipe,
                                             const float* __restrict__ bg, float* sOut, int outStride) {
     constexpr int WS = K + 4;
@@ -196,10 +196,7 @@ __device__ __forceinline__ void tile_linear(const float* sIn, int inStride, WPip
         float a[4] = {rowA[k0], rowB[k0], rowA[k0 + 4], rowB[k0 + 4]};
         uint32_t ah[4], al[4];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            if (RELU_IN) a[i] = fmaxf(a[i], 0.f);
-            split_tf32(a[i], ah[i], al[i]);
-        }
+        for (int i = 0; i < 4; ++i) split_tf32(a[i], ah[i], al[i]);
         uint32_t bh[NTW][2], bl[NTW][2];
 #pragma unroll
         for (int j = 0; j < NTW; ++j) {
@@ -216,7 +213,6 @@ __device__ __forceinline__ void tile_linear(const float* sIn, int inStride, WPip
         const int col = c0 + 8 * j + 2 * t;
         const float b0 = bias[j][0], b1 = bias[j][1];
         float v0 = acc[j][0] + b0, v1 = acc[j][1] + b1, v2 = acc[j][2] + b0, v3 = acc[j][3] + b1;
-        if (RELU_OUT) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
         sOut[(r0 + g) * outStride + col] = v0;
         sOut[(r0 + g) * outStride + col + 1] = v1;
         sOut[(r0 + g + 8) * outStride + col] = v2;
@@ -375,16 +371,7 @@ __global__ void __launch_bounds__(256, 3) hexplane_sample_kernel(SampleArgs a) {
     }
 }
 
-// load / store a [64][32L] tile of per-Gaussian rows between global memory and smem rows of stride FS
-__device__ __forceinline__ void tile_rows_load(const float* __restrict__ gsrc, int g0, int P, int FL, float* sDst, int FS) {
-    const int n4 = FL / 4;
-    for (int i = threadIdx.x; i < DT * n4; i += DTHREADS) {
-        const int g = i / n4, c4 = i - g * n4;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (g0 + g < P) v = __ldg(reinterpret_cast<const float4*>(gsrc + (size_t)(g0 + g) * FL) + c4);
-        *reinterpret_cast<float4*>(sDst + g * FS + 4 * c4) = v;
-    }
-}
+// store a [64][32L] tile of per-Gaussian rows from smem rows of stride FS to global memory
 __device__ __forceinline__ void tile_rows_store(float* __restrict__ gdst, int g0, int P, int FL, const float* sSrc, int FS) {
     const int n4 = FL / 4;
     for (int i = threadIdx.x; i < DT * n4; i += DTHREADS) {
@@ -562,7 +549,7 @@ struct DeformBwdArgs {
     float* gplanes[S3G_MAX_LEVELS][6];
     float* partial;      // [gridDim.x][off.total]
     const float* features;   // [P][32L] from the forward
-    const float* acts;       // hidden activations kept by the wgmma forward (SAVED kernels; layout: DeformTcArgs::acts), else NULL
+    const float* acts;       // hidden activations kept by the wgmma forward (layout: DeformTcArgs::acts)
     int act_slot[8];         // deform_host.cuh: AK_H, AK_POS, AK_SCL, AK_ROT, AK_OPA, AK_SHS, AK_D0, AK_D2; -1 = absent
     size_t act_stride;       // floats per slot = ceil(P / 128) * 128 * 64
     float* dfeatures;        // [P][32L] dL/d(features), consumed by hexplane_scatter_kernel
@@ -630,10 +617,10 @@ __device__ __forceinline__ void feat_layers_bwd(const DeformBwdSmem& sm, const D
     tile_linear_T<KF, 64, TL_ASSIGN>(sm.DH, HS, pipe, sm.A, FS, nullptr, 0);
 }
 
-// SAVED: the hidden activations (h and every head's hidden layer) come from the buffer the wgmma forward filled
-// instead of being recomputed - a third of the tile's MMA products and their barriers disappear; the tiles arrive by
-// cp.async one head ahead of their use, alternating between the two activation buffers.
-template <int LT, bool SAVED>
+// The hidden activations (h and every head's hidden layer) are read from the buffer the wgmma forward filled, so a
+// tile runs only the push-back products and the SH output layer; the stored tiles arrive by cp.async one head ahead
+// of their use, alternating between the two activation buffers.
+template <int LT>
 __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __grid_constant__ DeformBwdArgs a) {
     extern __shared__ __align__(16) float s_dyn[];
     const DNet& n = a.net;
@@ -648,7 +635,7 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
     WPipe pipe;
     pipe.start(a.wseq, &s_seq, sm.W, sm.W + HWID * (FS > HS ? FS : HS));
     __syncthreads();
-    // SAVED: which of the two activation buffers each stored tile lands in (consecutive enabled kinds alternate)
+    // which of the two activation buffers each stored tile lands in (consecutive enabled kinds alternate)
     const bool on_pos = n.pos.w1, on_scl = n.scl.w1, on_rot = n.rot.w1, on_opa = n.opa.w1, on_shs = n.shs.w1, on_d = n.w_d0;
     // The dino head needs its second hidden layer first, so that one travels a head ahead and takes the next
     // buffer in turn; the first hidden layer follows at the start of the head into the buffer the previous head used.
@@ -674,28 +661,16 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
 
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int g0 = tile * DT;
-        if (SAVED) {
-            // ---- h, the features (for the last product pair) and the first head's hidden layer: stored by the forward.
-            // The copies fly while the tile's scalars are set up; one barrier (after G below) covers all of it.
-            tile_canon_async(a.acts + (size_t)a.act_slot[0] * a.act_stride + (size_t)g0 * 64, sm.H, HS);
-            fetch_after(0, g0);
-            tile_rows_async(a.features, g0, a.P, FD * L, sm.F, FS);     // last group: only the final product pair reads it
-        }
+        // ---- h, the features (for the last product pair) and the first head's hidden layer: stored by the forward.
+        // The copies fly while the tile's scalars are set up; one barrier (after G below) covers all of it.
+        tile_canon_async(a.acts + (size_t)a.act_slot[0] * a.act_stride + (size_t)g0 * 64, sm.H, HS);
+        fetch_after(0, g0);
+        tile_rows_async(a.features, g0, a.P, FD * L, sm.F, FS);     // last group: only the final product pair reads it
         if (tid < DT * 3) {
             const int g = tid / 3, c = tid - 3 * g;
             sm.X[g * 4 + c] = (g0 + g < a.P) ? a.xyz[(size_t)(g0 + g) * 3 + c] : 0.f;
         }
         for (int i = tid; i < DT * HS; i += DTHREADS) sm.DH[i] = 0.f;
-        if (!SAVED) {
-        __syncthreads();
-        // ---- features of the tile (saved by the forward), hidden recomputed -------
-        tile_rows_load(a.features, g0, a.P, FD * L, sm.F, FS);
-        __syncthreads();
-        if (LT == 4 || L == 4) tile_linear<128, 64, false, false>(sm.F, FS, pipe, n.b_feat, sm.H, HS);
-        else if (L == 1) tile_linear<32, 64, false, false>(sm.F, FS, pipe, n.b_feat, sm.H, HS);
-        else if (L == 2) tile_linear<64, 64, false, false>(sm.F, FS, pipe, n.b_feat, sm.H, HS);
-        else if (L == 3) tile_linear<96, 64, false, false>(sm.F, FS, pipe, n.b_feat, sm.H, HS);
-        }
 
         // ---- per-Gaussian activation backward -> small deltas in G[g][0..10] ----
         //  G: [0..2] d(dx) , [3..5] d(ds), [6..9] d(dr), [10] d(do)
@@ -709,16 +684,15 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
                 for (int c = 0; c < 3; ++c) G[c] = ldz(a.g_means, (size_t)gi * 3 + c) + ldz(a.g_dx, (size_t)gi * 3 + c);
             }
         }
-        if (SAVED) asm volatile("cp.async.wait_group 1;" ::: "memory");      // everything but the features
+        asm volatile("cp.async.wait_group 1;" ::: "memory");      // everything but the features
         __syncthreads();
         // scales / rotation / opacity need their head outputs first (when the heads are on), so
         // the forward of those heads is recomputed into S-like columns of G[11..15] lazily below.
 
         // ---- pos head ------------------------------------------------------------
         if (n.pos.w1) {
-            float* Ab = SAVED ? abuf[1] : sm.A;
-            if (SAVED) fetch_after(1, g0);
-            else tile_linear<64, 64, true, true>(sm.H, HS, pipe, n.pos.b1, sm.A, HS);
+            float* Ab = abuf[1];
+            fetch_after(1, g0);
             if (tid < DT * 4) sm.Dout[tid] = sm.G[(tid >> 2) * 16 + (tid & 3)] * ((tid & 3) < 3 ? 1.f : 0.f);
             __syncthreads();
             small_head_backward(sm.Dout, 3, Ab, HS, n.pos.w2, part + a.off.pos[2], part + a.off.pos[3], sm.D1, HS);
@@ -728,10 +702,9 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
         // ---- scales head: scales_act = exp(scales + ds) ---------------------------
         {
             const bool on = n.scl.w1 != nullptr;
-            float* Ab = SAVED ? abuf[2] : sm.A;
+            float* Ab = abuf[2];
             if (on) {
-                if (SAVED) fetch_after(2, g0);
-                else tile_linear<64, 64, true, true>(sm.H, HS, pipe, n.scl.b1, sm.A, HS);
+                fetch_after(2, g0);
                 tile_small_out(Ab, HS, n.scl.w2, n.scl.b2, 3, sm.G, 16, 11);     // ds -> G[11..13]
                 __syncthreads();
             }
@@ -755,10 +728,9 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
         // ---- rotation head: rot_act = normalize(rot + dr) --------------------------
         {
             const bool on = n.rot.w1 != nullptr;
-            float* Ab = SAVED ? abuf[3] : sm.A;
+            float* Ab = abuf[3];
             if (on) {
-                if (SAVED) fetch_after(3, g0);
-                else tile_linear<64, 64, true, true>(sm.H, HS, pipe, n.rot.b1, sm.A, HS);
+                fetch_after(3, g0);
                 tile_small_out(Ab, HS, n.rot.w2, n.rot.b2, 4, sm.G, 16, 11);     // dr -> G[11..14]
                 __syncthreads();
             }
@@ -800,10 +772,9 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
         // ---- opacity head: opacity_act = sigmoid(opacity + do) ---------------------
         {
             const bool on = n.opa.w1 != nullptr;
-            float* Ab = SAVED ? abuf[4] : sm.A;
+            float* Ab = abuf[4];
             if (on) {
-                if (SAVED) fetch_after(4, g0);
-                else tile_linear<64, 64, true, true>(sm.H, HS, pipe, n.opa.b1, sm.A, HS);
+                fetch_after(4, g0);
                 tile_small_out(Ab, HS, n.opa.w2, n.opa.b2, 1, sm.G, 16, 11);     // do -> G[11]
                 __syncthreads();
             }
@@ -841,11 +812,10 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
                     pre_gd[i] = (a.g_dshs && idx < lim) ? __ldg(a.g_dshs + idx) : 0.f;
                 }
             }
-            float* Ab = SAVED ? abuf[5] : sm.A;
+            float* Ab = abuf[5];
             if (on) {
-                if (SAVED) fetch_after(5, g0);
-                else tile_linear<64, 64, true, true>(sm.H, HS, pipe, n.shs.b1, sm.A, HS);
-                tile_linear<64, 48, false, false>(Ab, HS, pipe, n.shs.b2, sm.Dout, 52);   // dshs
+                fetch_after(5, g0);
+                tile_linear<64, 48>(Ab, HS, pipe, n.shs.b2, sm.Dout, 52);   // dshs
             } else {
                 for (int i = tid; i < DT * 52; i += DTHREADS) sm.Dout[i] = 0.f;
                 __syncthreads();
@@ -956,20 +926,15 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
         }
         // ---- dino head ------------------------------------------------------------------
         if (n.w_d0) {
-            float* Ad = SAVED ? abuf[6] : sm.A;
-            float* Bd = SAVED ? abuf[7] : sm.B;
-            if (SAVED) {      // d2's layer arrived during the previous head; d0's (needed later) goes where that head's tile was
-                S3G_FETCH_ACT(6);
-            } else {
-                tile_linear<64, 64, false, true>(sm.H, HS, pipe, n.b_d0, sm.A, HS);
-                tile_linear<64, 64, false, true>(sm.A, HS, pipe, n.b_d2, sm.B, HS);
-            }
+            float* Ad = abuf[6];
+            float* Bd = abuf[7];
+            S3G_FETCH_ACT(6);      // d2's layer arrived during the previous head; d0's (needed later) goes where that head's tile was
             if (tid < DT * 4) {
                 const int g = tid >> 2, c = tid & 3, gi = g0 + g;
                 sm.Dout[tid] = (c < 3 && gi < a.P) ? ldz(a.g_feat, (size_t)gi * 3 + c) : 0.f;
             }
             __syncthreads();
-            small_head_backward(sm.Dout, 3, Bd, HS, n.w_d4, part + a.off.d4w, part + a.off.d4b, sm.D2, HS, SAVED);
+            small_head_backward(sm.Dout, 3, Bd, HS, n.w_d4, part + a.off.d4w, part + a.off.d4b, sm.D2, HS, true);
             dw_accum<64, 64, false>(sm.D2, HS, Ad, HS, part + a.off.d2w, part + a.off.d2b);
             tile_linear_T<64, 64, TL_ASSIGN_MASK>(sm.D2, HS, pipe, sm.D1, HS, Ad, HS);
             dw_accum<64, 64, false>(sm.D1, HS, sm.H, HS, part + a.off.d0w, part + a.off.d0b);

@@ -53,27 +53,18 @@ inline int to_dnet(const s3g_deform_net* n, DNet& d) {
         return fail(S3G_ERR_ARG, "deform: incomplete dino head");
     return S3G_OK;
 }
-// weight matrices in the order one tile consumes them (see WPipe).  `saved`: the backward reads the hidden
-// activations the forward stored instead of recomputing them, so only the push-back products (and the 48-wide SH
-// output layer, whose result is not stored) remain.
-inline void build_wseq(const DNet& d, bool backward, WSeq& q, bool saved = false) {
+// weight matrices in the order one backward tile consumes them (see WPipe).  The backward reads the hidden
+// activations the forward stored, so only the push-back products (and the 48-wide SH output layer, whose result is
+// not stored) use weights.
+inline void build_wseq(const DNet& d, WSeq& q) {
     q.count = 0;
     auto add = [&](const float* W, int N, int K) { q.W[q.count] = W; q.N[q.count] = (short)N; q.K[q.count] = (short)K; ++q.count; };
-    const int KF = FD * d.L;
-    if (!saved) add(d.w_feat, 64, KF);
     const Head2* small[4] = {&d.pos, &d.scl, &d.rot, &d.opa};
     for (const Head2* h : small)
-        if (h->w1) { if (!saved) add(h->w1, 64, 64); if (backward) add(h->w1, 64, 64); }
-    if (d.shs.w1) {
-        if (!saved) add(d.shs.w1, 64, 64);
-        add(d.shs.w2, 48, 64);
-        if (backward) { add(d.shs.w2, 48, 64); add(d.shs.w1, 64, 64); }
-    }
-    if (d.w_d0) {
-        if (!saved) { add(d.w_d0, 64, 64); add(d.w_d2, 64, 64); }
-        if (backward) { add(d.w_d2, 64, 64); add(d.w_d0, 64, 64); }
-    }
-    if (backward) add(d.w_feat, 64, KF);
+        if (h->w1) add(h->w1, 64, 64);
+    if (d.shs.w1) { add(d.shs.w2, 48, 64); add(d.shs.w2, 48, 64); add(d.shs.w1, 64, 64); }
+    if (d.w_d0) { add(d.w_d2, 64, 64); add(d.w_d0, 64, 64); }
+    add(d.w_feat, 64, FD * d.L);
 }
 
 // Hidden activations the wgmma forward can keep for the backward: [slot][P][64] floats, one slot per enabled

@@ -71,12 +71,6 @@ def _p(t):
     return None if t is None else t.data_ptr()
 
 
-# True: the forward keeps the decoder's hidden activations for the backward (s3g_deform_forward_save /
-# s3g_deform_backward_saved, 256 B per Gaussian and hidden layer).  False: the backward recomputes them from the
-# sampled features (s3g_deform_backward), which trades backward time for that memory.
-SAVE_ACTIVATIONS = True
-
-
 class HexPlaneField(nn.Module):
     """Parameter container with the reference's names (scene/hexplane.py:109-158)."""
 
@@ -319,10 +313,9 @@ class _DeformFront(torch.autograd.Function):
         features = e(P, 32 * len(module.deformation_net.grid.grids))     # sampler -> decoder hand-over, kept for backward
         campos_ = campos.detach().to(device=dev, dtype=torch.float32).contiguous()
         fws = torch.empty(int(lib.s3g_deform_forward_workspace_bytes(C.byref(cnet))), dtype=torch.uint8, device=dev)
-        # when a backward will follow, the decoder's hidden activations are kept (what autograd keeps for the reference's
-        # nn.Sequential heads) so that the backward kernel does not recompute them (opaque buffer, 256 B per Gaussian
-        # and hidden layer)
-        nbytes = int(lib.s3g_deform_saved_bytes(C.byref(cnet), P)) if (SAVE_ACTIVATIONS and any(ctx.needs_input_grad)) else 0
+        # when a backward will follow, the decoder's hidden activations are kept for it (what autograd keeps for the
+        # reference's nn.Sequential heads; opaque buffer, 256 B per Gaussian and hidden layer)
+        nbytes = int(lib.s3g_deform_saved_bytes(C.byref(cnet), P)) if any(ctx.needs_input_grad) else 0
         acts = torch.empty(nbytes, dtype=torch.uint8, device=dev) if nbytes > 0 else None
         with torch.cuda.device(dev):
             _lib.check(lib.s3g_deform_forward_save(C.byref(cnet), P, _p(xyz_), _p(sc_), _p(ro_), _p(op_), _p(shs_),
@@ -337,18 +330,14 @@ class _DeformFront(torch.autograd.Function):
                 raise NotImplementedError("forward_dynamic with scale/rotation/opacity heads: use render_front()")
             sc_o, ro_o, op_o = sc_.clone(), ro_.clone(), op_.clone()
         ctx.module, ctx.time, ctx.sh_degree, ctx.raw, ctx.names = module, float(time), int(sh_degree), raw_outputs, names
-        ctx.has_acts = acts is not None
-        ctx.save_for_backward(xyz_, sc_, ro_, op_, shs_, campos_, features, acts if acts is not None else torch.empty(0, dtype=torch.uint8, device=dev),
-                              *[p.detach() for p in params])
+        ctx.save_for_backward(xyz_, sc_, ro_, op_, shs_, campos_, features, acts, *[p.detach() for p in params])
         return means, sc_o, ro_o, op_o, colors, dx, dshs, feat
 
     @staticmethod
     def backward(ctx, g_means, g_sc, g_ro, g_op, g_col, g_dx, g_dshs, g_feat):
         lib = _lib.load()
         module = ctx.module
-        xyz, sc, ro, op, shs, campos, features, acts, *params = ctx.saved_tensors
-        if not ctx.has_acts:
-            acts = None
+        xyz, sc, ro, op, shs, campos, features, acts, *params = ctx.saved_tensors     # acts is None only when P == 0
         dev = xyz.device
         P = xyz.shape[0]
         byname = dict(zip(ctx.names, params))

@@ -96,3 +96,20 @@ def test_saved_activation_buffer_size_follows_the_enabled_heads(built_lib):
     assert saved(nofeat, 300) == 2 * per_slot(300)
     deep = make(reso=(8, 8, 8, 5), multires=(1, 2, 3, 4, 5))   # 5 levels: not a supported net -> 0, and the forward raises
     assert saved(deep, 1000) == 0
+
+
+def test_backward_without_saved_activations_is_an_argument_error(built_lib):
+    """s3g_deform_backward_saved reads the hidden activations the forward kept: with P > 0 a NULL `acts` returns
+    S3G_ERR_ARG with a message, before any CUDA call (so no GPU is needed here)."""
+    import ctypes as C
+    from s3gaussian_b200.deformation import CNet, CNetGrads
+    net = make()
+    byname = {n: p.detach() for n, p in net._named_hot_params()}
+    grads = {n: torch.zeros_like(p) for n, p in byname.items()}
+    cnet, cg = CNet(), CNetGrads()
+    net._fill(cnet, byname, grads=(cg, grads))
+    dummy = C.c_void_p(256)      # never dereferenced: the call returns before it touches a device pointer
+    rc = built_lib.s3g_deform_backward_saved(C.byref(cnet), 100, *[dummy] * 5, 0.5, dummy, 3, dummy, None,
+                                             *[None] * 8, *[dummy] * 5, C.byref(cg), dummy, None)
+    assert rc == -1
+    assert b"null acts" in built_lib.s3g_last_error()

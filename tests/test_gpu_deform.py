@@ -29,13 +29,10 @@ def build_net(z, st, flags):
     return net.to(DEV)
 
 
-@pytest.mark.parametrize("saved", [True, False], ids=["saved_activations", "recompute"])
 @pytest.mark.parametrize("path", GOLD, ids=[os.path.basename(p)[7:-4] for p in GOLD])
-def test_fused_deform_matches_reference_golden(path, saved, built_lib, monkeypatch):
-    """both backward variants against the reference's golden gradients: hidden activations kept by the wgmma
-    forward (s3g_deform_forward_save / s3g_deform_backward_saved) and recomputed in the backward kernel"""
-    from s3gaussian_b200 import deformation
-    monkeypatch.setattr(deformation, "SAVE_ACTIVATIONS", saved)
+def test_fused_deform_matches_reference_golden(path, built_lib):
+    """outputs and gradients against the reference's golden vectors; the backward reads the hidden activations
+    the wgmma forward kept (s3g_deform_forward_save / s3g_deform_backward_saved)"""
     z, st, flags = load_deform_case(path)
     net = build_net(z, st, flags)
     T = lambda k: torch.from_numpy(z[k]).to(DEV).requires_grad_(True)
@@ -69,17 +66,15 @@ def test_fused_deform_matches_reference_golden(path, saved, built_lib, monkeypat
     assert checked >= 28
 
 
-@pytest.mark.parametrize("saved", [True, False], ids=["saved_activations", "recompute"])
 @pytest.mark.parametrize("L", [1, 2, 3, 4])
-def test_level_counts_against_the_oracle(L, saved, built_lib, monkeypatch):
+def test_level_counts_against_the_oracle(L, built_lib):
     """1 .. 4 HexPlane levels (the level counts the kernels accept; feature widths 32 .. 128): the wgmma forward
     runs the feature layer as K-halves of 32+0, 64+0, 64+32 and 64+64 columns, the backward's generic-L
     instantiations cover 1 .. 3.  Forward
     outputs and every gradient against oracle/deform_oracle.py (float64 torch autograd), all heads enabled."""
     from oracle import deform_oracle as do
-    from s3gaussian_b200 import deformation, synthetic as syn
+    from s3gaussian_b200 import synthetic as syn
     from s3gaussian_b200.deformation import deform_network
-    monkeypatch.setattr(deformation, "SAVE_ACTIVATIONS", saved)
     reso, multires = (12, 10, 8, 6), tuple(range(1, L + 1))
     aabb = ((9.0, 4.0, 3.0), (-2.0, -4.0, -3.0))
     flags = dict(no_ds=False, no_dr=False, no_do=False)

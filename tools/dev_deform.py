@@ -17,9 +17,6 @@ def make_args(reso, multires, **flags):
     d.update(flags); return Namespace(**d)
 
 dev = torch.device("cuda:0")
-if "--recompute" in sys.argv:
-    from s3gaussian_b200 import deformation as _d
-    _d.SAVE_ACTIVATIONS = False
 do_bwd = "--bwd" in sys.argv
 for path in ([] if "--notest" in sys.argv else sorted(glob.glob(os.path.join(ROOT, "tests", "golden", "deform_*.npz")))):
     z, st, flags = load_deform_case(path)
