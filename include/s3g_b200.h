@@ -387,6 +387,33 @@ size_t s3g_lpips_alex_workspace_bytes(int N, int H, int W);
 int s3g_lpips_alex(int N, int H, int W, const float* x, const float* y, const void* prepared, double* out,
                    void* workspace, void* stream);
 
+/* LPIPS backward: the gradients of s3g_lpips_alex's out[6] with respect to x and / or y (the weights are frozen, as
+ * in lpipsPyTorch).  grad_out: DEVICE double [6], the upstream gradient of out; layer l's taps are weighed by
+ * grad_out[l] + grad_out[5], so any mix of the layer terms and the total differentiates correctly.
+ *
+ * s3g_lpips_alex_backward_prepare: once per model, after or independently of s3g_lpips_alex_prepare, writes the
+ * backward's weight layout into `prepared_bwd` (DEVICE, s3g_lpips_alex_backward_prepared_bytes(), 16-byte aligned):
+ * conv 1's weights as given and, for convolutions 2-5, the flipped and transposed kernels as tf32 hi/lo tiles.  Only
+ * weights->conv_w is read.
+ *
+ * s3g_lpips_alex_backward: N, H, W, `prepared` are those of the s3g_lpips_alex call being differentiated, and
+ * fwd_workspace MUST be that call's workspace, unchanged since: the backward reads the saved activations (every
+ * ReLU output, for the masks, the taps and the max-pool argmaxes) and never the images.  grad_x / grad_y: DEVICE
+ * float [N,3,H,W], written (not accumulated); NULL = not wanted, and the work of that side is skipped.
+ * workspace: s3g_lpips_alex_backward_workspace_bytes(N, H, W) bytes (0 for invalid sizes), about 0.1 GB for one
+ * 1920x1280 pair.  No host synchronisation; deterministic: no atomics, two calls give bitwise equal gradients.
+ * The dgrads of convolutions 2-5 are implicit GEMMs on the tensor cores in the forward's 3xTF32 arithmetic; conv 1's
+ * (3 output channels) runs on the CUDA cores in fp32.
+ * S3G_ERR_ARG before any launch: the size rules of s3g_lpips_alex, a null prepared / prepared_bwd / fwd_workspace /
+ * grad_out / workspace, both gradients NULL, or an unaligned buffer (prepared and prepared_bwd 16 bytes, grad_out 8,
+ * grad_x / grad_y 4). */
+size_t s3g_lpips_alex_backward_prepared_bytes(void);
+int s3g_lpips_alex_backward_prepare(const s3g_lpips_alex_weights* weights, void* prepared_bwd, void* stream);
+size_t s3g_lpips_alex_backward_workspace_bytes(int N, int H, int W);
+int s3g_lpips_alex_backward(int N, int H, int W, const void* prepared, const void* prepared_bwd,
+                            const void* fwd_workspace, const double* grad_out, float* grad_x, float* grad_y,
+                            void* workspace, void* stream);
+
 /* ---- state-buffer introspection (tests / debugging) ---------------------
  * buffer: 0 = geometry, 1 = binning, 2 = image.  Looks up a named field of our
  * layout for the given problem size and returns its byte offset from the

@@ -49,6 +49,10 @@ SIGNATURES = {
     "s3g_lpips_alex_prepare": (_I, [_V, _V, _V]),
     "s3g_lpips_alex_workspace_bytes": (_SZ, [_I, _I, _I]),
     "s3g_lpips_alex": (_I, [_I, _I, _I, _V, _V, _V, _V, _V, _V]),
+    "s3g_lpips_alex_backward_prepared_bytes": (_SZ, []),
+    "s3g_lpips_alex_backward_prepare": (_I, [_V, _V, _V]),
+    "s3g_lpips_alex_backward_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "s3g_lpips_alex_backward": (_I, [_I, _I, _I, _V, _V, _V, _V, _V, _V, _V, _V]),
     "s3g_rasterize_backward_dp": (_I, [_I, _I, _I, _I64, _V, _I, _I, _V, _V, _V, _V, _F, _V, _V, _V, _V,
                                        _V, _F, _F, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V, _V,
                                        _V, _V, _V, _I, _V, _V]),

@@ -64,6 +64,64 @@ bool args_ok(int N, int H, int W) {
     return N >= 1 && H >= 31 && W >= 31 && (int64_t)N * 3 * H * W < INT32_MAX && LpShapes(N, H, W).fits_int32();
 }
 
+// float offsets inside the backward's prepared buffer: conv 1's weights as given ([64][3][11][11], read by the CUDA
+// core dgrad), then the dgrad tiles of convolutions 2-5
+struct LpPreparedBwd {
+    size_t w0, tiles[LP_LAYERS], total;
+    LpPreparedBwd() {
+        size_t o = 0;
+        w0 = o; o += (size_t)lp_cout(0) * lp_k(0);
+        tiles[0] = 0;
+        for (int l = 1; l < LP_LAYERS; ++l) { tiles[l] = o; o += (size_t)lp_tiles(l) * LP_TILE_FLOATS; }
+        total = o;
+    }
+};
+
+// The backward's two ping-pong gradient buffers, sized for all 2N images.  Going down, A holds the gradients at
+// conv 5, 3 and 2's outputs and at conv 1's, B those at conv 4's output and at the two max-pool outputs.
+struct LpBwdShapes {
+    size_t a_off, b_off, bytes;
+    explicit LpBwdShapes(const LpShapes& s) {
+        const int64_t a = std::max({s.conv_elems[4], s.conv_elems[2], s.conv_elems[1], s.conv_elems[0]});
+        const int64_t b = std::max({s.conv_elems[3], s.pool_elems[1], s.pool_elems[0]});
+        a_off = 0;
+        b_off = ((size_t)a * 4 + 255) & ~(size_t)255;
+        bytes = b_off + (((size_t)b * 4 + 255) & ~(size_t)255) + 256;   // + alignment of the base
+    }
+};
+
+template <int L>
+int launch_dgrad(const LpConvArgs& a, cudaStream_t stream) {
+    S3G_CUDA(cudaFuncSetAttribute(lpips_dgrad_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, LP_SMEM_BYTES),
+             "lpips dgrad smem attribute");
+    const dim3 grid((unsigned)div_up64(a.M, LP_BM), lp_cin(L) / LP_BN);
+    lpips_dgrad_kernel<L><<<grid, LP_THREADS, LP_SMEM_BYTES, stream>>>(a);
+    S3G_CUDA(cudaGetLastError(), "lpips dgrad launch");
+    return S3G_OK;
+}
+
+template <int C>
+int launch_tap_bwd(int P, int layer, double pixels, int wx, int wy, int accumulate, const float* f, const float* lin,
+                   const double* gout, float* g, cudaStream_t stream) {
+    const int64_t blocks = div_up64(P, LP_TAP_WARPS * LP_TAP_PIX);
+    lpips_tap_bwd_kernel<C><<<(unsigned)blocks, 32 * LP_TAP_WARPS, 0, stream>>>(P, layer, pixels, wx, wy, accumulate, f,
+                                                                               lin, gout, g);
+    S3G_CUDA(cudaGetLastError(), "lpips tap backward launch");
+    return S3G_OK;
+}
+
+int tap_bwd(int l, int P, double pixels, int wx, int wy, int accumulate, const float* f, const float* lin,
+            const double* gout, float* g, cudaStream_t stream) {
+    switch (lp_cout(l)) {
+        case 64: return launch_tap_bwd<64>(P, l, pixels, wx, wy, accumulate, f, lin, gout, g, stream);
+        case 192: return launch_tap_bwd<192>(P, l, pixels, wx, wy, accumulate, f, lin, gout, g, stream);
+        case 384: return launch_tap_bwd<384>(P, l, pixels, wx, wy, accumulate, f, lin, gout, g, stream);
+        default: return launch_tap_bwd<256>(P, l, pixels, wx, wy, accumulate, f, lin, gout, g, stream);
+    }
+}
+
+bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+
 template <int L>
 int launch_conv(const LpConvArgs& a, cudaStream_t stream) {
     S3G_CUDA(cudaFuncSetAttribute(lpips_conv_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, LP_SMEM_BYTES),
@@ -182,6 +240,118 @@ int s3g_lpips_alex(int N, int H, int W, const float* x, const float* y, const vo
     r.out = out;
     lpips_reduce_kernel<<<1, 256, 0, stream>>>(r);
     S3G_CUDA(cudaGetLastError(), "lpips reduce launch");
+    return S3G_OK;
+}
+
+size_t s3g_lpips_alex_backward_prepared_bytes(void) { return LpPreparedBwd().total * sizeof(float); }
+
+int s3g_lpips_alex_backward_prepare(const s3g_lpips_alex_weights* wts, void* prepared_bwd, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (!wts || !prepared_bwd) return fail(S3G_ERR_ARG, "lpips_alex_backward_prepare: null weights/prepared_bwd");
+    for (int l = 0; l < LP_LAYERS; ++l)
+        if (!wts->conv_w[l]) return fail(S3G_ERR_ARG, "lpips_alex_backward_prepare: null convolution weight pointer");
+    if (!aligned(prepared_bwd, 16))
+        return fail(S3G_ERR_ARG, "lpips_alex_backward_prepare: prepared_bwd must be 16-byte aligned");
+    const LpPreparedBwd lay;
+    float* dst = static_cast<float*>(prepared_bwd);
+    S3G_CUDA(cudaMemcpyAsync(dst + lay.w0, wts->conv_w[0], (size_t)lp_cout(0) * lp_k(0) * sizeof(float),
+                             cudaMemcpyDeviceToDevice, stream), "lpips_alex_backward_prepare conv 1 copy");
+    LpPrepArgs p{};
+    for (int l = 1; l < LP_LAYERS; ++l) {
+        p.w[l] = wts->conv_w[l];
+        p.dst[l] = dst + lay.tiles[l];
+    }
+    lpips_prep_dgrad_kernel<<<dim3(256, LP_LAYERS - 1), 256, 0, stream>>>(p);
+    S3G_CUDA(cudaGetLastError(), "lpips_prep_dgrad launch");
+    return S3G_OK;
+}
+
+size_t s3g_lpips_alex_backward_workspace_bytes(int N, int H, int W) {
+    if (!args_ok(N, H, W)) return 0;
+    return LpBwdShapes(LpShapes(N, H, W)).bytes;
+}
+
+int s3g_lpips_alex_backward(int N, int H, int W, const void* prepared, const void* prepared_bwd,
+                            const void* fwd_workspace, const double* grad_out, float* grad_x, float* grad_y,
+                            void* workspace, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (N < 1) return fail(S3G_ERR_ARG, "lpips_alex_backward: N >= 1 images expected");
+    if (H < 31 || W < 31) return fail(S3G_ERR_ARG, "lpips_alex_backward: image sides must be >= 31");
+    if (!args_ok(N, H, W)) return fail(S3G_ERR_ARG, "lpips_alex_backward: images too large for 32-bit indices");
+    if (!prepared || !prepared_bwd || !fwd_workspace || !grad_out || !workspace)
+        return fail(S3G_ERR_ARG, "lpips_alex_backward: null prepared/prepared_bwd/fwd_workspace/grad_out/workspace");
+    if (!grad_x && !grad_y) return fail(S3G_ERR_ARG, "lpips_alex_backward: neither grad_x nor grad_y requested");
+    if (!aligned(prepared, 16) || !aligned(prepared_bwd, 16) || !aligned(grad_out, 8) || !aligned(grad_x, 4) ||
+        !aligned(grad_y, 4))
+        return fail(S3G_ERR_ARG, "lpips_alex_backward: unaligned prepared/prepared_bwd (16), grad_out (8) or grad (4)");
+    const LpShapes s(N, H, W);
+    const LpBwdShapes bs(s);
+    const LpPrepared lay;
+    const LpPreparedBwd blay;
+    const float* wp = static_cast<const float*>(prepared);
+    const float* wb = static_cast<const float*>(prepared_bwd);
+    // the forward's layout (s3g_lpips_alex): same base rounding, same offsets
+    const char* fbase = reinterpret_cast<const char*>(((uintptr_t)fwd_workspace + 255) & ~(uintptr_t)255);
+    auto saved = [&](size_t off) { return reinterpret_cast<const float*>(fbase + off); };
+    char* base = reinterpret_cast<char*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+    float* ga = reinterpret_cast<float*>(base + bs.a_off);
+    float* gb = reinterpret_cast<float*>(base + bs.b_off);
+
+    const int wx = grad_x != nullptr, wy = grad_y != nullptr;
+    const int NB = (wx + wy) * N;          // images with a gradient: rows of every buffer below
+    const int64_t i0 = wx ? 0 : N;          // ... starting at this image of the forward's 2N
+    auto tap = [&](int l, int accumulate, float* g) {
+        return tap_bwd(l, (int)(N * s.h[l] * s.w[l]), (double)(s.h[l] * s.w[l]), wx, wy, accumulate,
+                       saved(s.conv_off[l]), wp + lay.lin[l], grad_out, g, stream);
+    };
+    auto dgrad = [&](int l, const float* dy, float* dx) {
+        LpConvArgs a{};
+        a.in = dy; a.N = NB; a.H = a.Ho = (int)s.h[l]; a.W = a.Wo = (int)s.w[l];
+        a.M = NB * a.Ho * a.Wo;
+        a.wprep = wb + blay.tiles[l];
+        a.out = dx;
+        switch (l) {
+            case 1: return launch_dgrad<1>(a, stream);
+            case 2: return launch_dgrad<2>(a, stream);
+            case 3: return launch_dgrad<3>(a, stream);
+            default: return launch_dgrad<4>(a, stream);
+        }
+    };
+    // gradient at pool p's output (dout) -> gradient at conv p's output (din), argmaxes from the saved conv output
+    auto pool = [&](int p, const float* dout, float* din) {
+        const int C4 = lp_cout(p) / 4;
+        const int64_t total4 = (int64_t)NB * s.h[p] * s.w[p] * C4;
+        const int grid = (int)std::min<int64_t>(div_up64(total4, 256), (int64_t)device_sm_count() * 16);
+        const float* in = saved(s.conv_off[p]) + i0 * s.h[p] * s.w[p] * lp_cout(p);
+        lpips_maxpool_bwd_kernel<<<grid, 256, 0, stream>>>((int)total4, C4, (int)s.h[p], (int)s.w[p], (int)s.ph[p],
+                                                            (int)s.pw[p], reinterpret_cast<const float4*>(in),
+                                                            reinterpret_cast<const float4*>(dout),
+                                                            reinterpret_cast<float4*>(din));
+        S3G_CUDA(cudaGetLastError(), "lpips maxpool backward launch");
+        return S3G_OK;
+    };
+    int rc;
+    if ((rc = tap(4, 0, ga)) != S3G_OK) return rc;
+    if ((rc = dgrad(4, ga, gb)) != S3G_OK) return rc;
+    if ((rc = tap(3, 1, gb)) != S3G_OK) return rc;
+    if ((rc = dgrad(3, gb, ga)) != S3G_OK) return rc;
+    if ((rc = tap(2, 1, ga)) != S3G_OK) return rc;
+    if ((rc = dgrad(2, ga, gb)) != S3G_OK) return rc;
+    if ((rc = pool(1, gb, ga)) != S3G_OK) return rc;
+    if ((rc = tap(1, 1, ga)) != S3G_OK) return rc;
+    if ((rc = dgrad(1, ga, gb)) != S3G_OK) return rc;
+    if ((rc = pool(0, gb, ga)) != S3G_OK) return rc;
+    if ((rc = tap(0, 1, ga)) != S3G_OK) return rc;
+
+    LpDgrad0Args d{};
+    d.dy = ga; d.w = wb + blay.w0;
+    d.first = wx ? grad_x : grad_y; d.second = grad_y;
+    d.N = N; d.H = H; d.W = W; d.Ho = (int)s.h[0]; d.Wo = (int)s.w[0];
+    d.tiles_x = (int)div_up64(div_up64(W, 4), LP_D0_TX);
+    d.tiles_y = (int)div_up64(div_up64(H, 4), LP_D0_TY);
+    const int64_t blocks = (int64_t)NB * 16 * d.tiles_x * d.tiles_y;
+    lpips_dgrad0_kernel<<<(unsigned)blocks, dim3(LP_D0_TX, LP_D0_TY), 0, stream>>>(d);
+    S3G_CUDA(cudaGetLastError(), "lpips dgrad0 launch");
     return S3G_OK;
 }
 

@@ -85,6 +85,29 @@ __global__ void __launch_bounds__(256) lpips_prep_kernel(const __grid_constant__
     }
 }
 
+// Dgrad weights of convolutions 1..4 (blockIdx.y + 1): B'[ci][k'] with k' = (ky', kx', co) is
+// w[co][ci][KS-1-ky'][KS-1-kx'], the flipped, transposed kernel, as [Cin / 64][KS*KS*Cout / 32] hi | lo tiles
+// (lpips_dgrad_kernel's K order: 32 consecutive output channels of one tap per chunk).  Layer 0's dgrad runs on the
+// CUDA cores from the PyTorch layout (lpips_dgrad0_kernel).
+__global__ void __launch_bounds__(256) lpips_prep_dgrad_kernel(const __grid_constant__ LpPrepArgs p) {
+    const int l = blockIdx.y + 1;
+    const int Cin = lp_cin(l), Cout = lp_cout(l), KS = lp_ks(l), K = KS * KS * Cout, KC = K / LP_BK;
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < Cin * K; e += gridDim.x * blockDim.x) {
+        const int ci = e / K, k = e - ci * K;
+        const int tap = k / Cout, co = k - tap * Cout;
+        const int ky = KS - 1 - tap / KS, kx = KS - 1 - tap % KS;
+        const float v = __ldg(p.w[l] + (((size_t)co * Cin + ci) * KS + ky) * KS + kx);
+        uint32_t hi, lo;
+        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(v));
+        const float r = v - __uint_as_float(hi);
+        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(r));
+        float* t = p.dst[l] + (size_t)((ci / LP_BN) * KC + k / LP_BK) * LP_TILE_FLOATS;
+        const int idx = umma::canon_idx(ci % LP_BN, k % LP_BK, LP_BK);
+        t[idx] = __uint_as_float(hi);
+        t[LP_B_FLOATS + idx] = __uint_as_float(lo);
+    }
+}
+
 // ---- convolution -------------------------------------------------------------------------------------------------
 struct LpConvArgs {
     const float* in;        // layers 2-5: [2N][H][W][Cin] channels-last
@@ -103,10 +126,15 @@ __device__ __forceinline__ void lp_cp16(float* sdst, const float* gsrc) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(umma::smem_u32(sdst)), "l"(gsrc) : "memory");
 }
 
-template <int L>
-__global__ void __launch_bounds__(LP_THREADS, 2) lpips_conv_kernel(const __grid_constant__ LpConvArgs a) {
-    constexpr int Cin = lp_cin(L), Cout = lp_cout(L), KS = lp_ks(L), S = lp_stride(L), PAD = lp_pad(L);
-    constexpr int K = lp_k(L), KC = lp_kpad(L) / LP_BK;
+// One 128 x 64 output tile of convolution L (DG = false), or of the input gradient of convolution L >= 1 (DG = true).
+// The dgrad of a stride-1 "same" convolution is itself one: input dY [NI][H][W][Cout], output dX [NI][H][W][Cin],
+// the same KS and PAD, the kernel flipped and transposed (lpips_prep_dgrad_kernel), no bias and no ReLU.
+template <int L, bool DG>
+__device__ __forceinline__ void lp_conv_tile(const LpConvArgs& a) {
+    static_assert(!DG || (L > 0 && lp_stride(L) == 1 && 2 * lp_pad(L) == lp_ks(L) - 1), "dgrad: stride-1 same conv");
+    constexpr int Cin = DG ? lp_cout(L) : lp_cin(L), Cout = DG ? lp_cin(L) : lp_cout(L);
+    constexpr int KS = lp_ks(L), S = lp_stride(L), PAD = lp_pad(L);
+    constexpr int K = KS * KS * Cin, KC = (K + LP_BK - 1) / LP_BK;
     constexpr uint32_t SBO = (LP_BK / 4) * 128u, MHALF = 8u * SBO;
     extern __shared__ __align__(128) float s_lp[];
     const int tid = threadIdx.x;
@@ -119,13 +147,13 @@ __global__ void __launch_bounds__(LP_THREADS, 2) lpips_conv_kernel(const __grid_
     const int iy0 = oy * S - PAD, ix0 = ox * S - PAD;
     const float* wtiles = a.wprep + (size_t)blockIdx.y * KC * LP_TILE_FLOATS;
     const float* src = nullptr;     // layer 1: channel 0 of this pixel's image
-    if constexpr (L == 0) src = (img < a.N ? a.x + (size_t)img * 3 * a.H * a.W : a.y + (size_t)(img - a.N) * 3 * a.H * a.W);
+    if constexpr (!DG && L == 0) src = (img < a.N ? a.x + (size_t)img * 3 * a.H * a.W : a.y + (size_t)(img - a.N) * 3 * a.H * a.W);
 
     // this thread's 32 A values of chunk c (zero outside the image, past K and past M)
     float v[LP_BK];
     auto gather = [&](int c) {
         const int k0 = c * LP_BK;
-        if constexpr (L == 0) {
+        if constexpr (!DG && L == 0) {
 #pragma unroll
             for (int j = 0; j < LP_BK; ++j) {
                 const int k = k0 + j;
@@ -204,7 +232,7 @@ __global__ void __launch_bounds__(LP_THREADS, 2) lpips_conv_kernel(const __grid_
         umma::wgmma_wait_all();
         umma::fence_regs(acc[0]); umma::fence_regs(acc[1]);
     }
-    // epilogue: + bias, ReLU, channels-last store (fragment layout, umma.cuh)
+    // epilogue: + bias, ReLU (forward only), channels-last store (fragment layout, umma.cuh)
     const int n0 = blockIdx.y * LP_BN;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -213,12 +241,26 @@ __global__ void __launch_bounds__(LP_THREADS, 2) lpips_conv_kernel(const __grid_
             const int row = blockIdx.x * LP_BM + 64 * h + umma::frag_row(i);
             const int col = n0 + umma::frag_col(i);
             if (row < a.M) {
-                const float b0 = __ldg(a.bias + col), b1 = __ldg(a.bias + col + 1);
-                *reinterpret_cast<float2*>(a.out + (size_t)row * Cout + col) =
-                    make_float2(fmaxf(acc[h][i] + b0, 0.f), fmaxf(acc[h][i + 1] + b1, 0.f));
+                float2 o = make_float2(acc[h][i], acc[h][i + 1]);
+                if constexpr (!DG) {
+                    const float b0 = __ldg(a.bias + col), b1 = __ldg(a.bias + col + 1);
+                    o = make_float2(fmaxf(o.x + b0, 0.f), fmaxf(o.y + b1, 0.f));
+                }
+                *reinterpret_cast<float2*>(a.out + (size_t)row * Cout + col) = o;
             }
         }
     }
+}
+
+template <int L>
+__global__ void __launch_bounds__(LP_THREADS, 2) lpips_conv_kernel(const __grid_constant__ LpConvArgs a) {
+    lp_conv_tile<L, false>(a);
+}
+
+// dX of convolution L (1..4) from dY; a.in = dY, a.out = dX, a.M = images * H * W, a.wprep = the dgrad tiles
+template <int L>
+__global__ void __launch_bounds__(LP_THREADS, 2) lpips_dgrad_kernel(const __grid_constant__ LpConvArgs a) {
+    lp_conv_tile<L, true>(a);
 }
 
 // ---- max-pool 3/2, no padding, floor mode, channels-last [NI][H][W][C] -> [NI][Ho][Wo][C] ---------------------------
@@ -323,6 +365,179 @@ __global__ void __launch_bounds__(256) lpips_reduce_kernel(const __grid_constant
         __syncthreads();
     }
     if (threadIdx.x == 0) r.out[LP_LAYERS] = total;
+}
+
+// ==== backward ====================================================================================================
+// The gradients of the images that need one: NB = N (x's or y's) or 2N (x's then y's) rows of every buffer, at image
+// i0 = 0 or N of the forward's 2N.  From the top: tap 5 -> dgrad 5 -> tap 4 -> dgrad 4 -> tap 3 -> dgrad 3 -> pool 2
+// -> tap 2 -> dgrad 2 -> pool 1 -> tap 1 -> layer-1 dgrad into the caller's CHW images.
+
+// Tap l's gradient, added to the gradient g already there (unless `accumulate` is 0) and masked by the ReLU:
+// g <- (f > 0) ? g + d tap / d f : 0, in place, channels-last rows.  One warp per pixel pair p < P = N * Hl * Wl, as
+// the forward tap.  With a = f / D, D = |f| + 1e-10 and G = gout[l] + gout[5]:
+//   u = G * 2 * lin * (a_x - a_y) / (Hl * Wl)   (-u on the y side),   d/df = u / D - f (u.f) / (|f| D^2)
+// A zero feature vector gets 0 (its whole row is masked; torch's threshold_backward zeroes the reference's 0/0).
+// x's row p is row p of g when wx; y's row p is row (wx ? P : 0) + p when wy.  f holds all 2N images.
+template <int C>
+__global__ void __launch_bounds__(32 * LP_TAP_WARPS) lpips_tap_bwd_kernel(int P, int layer, double pixels, int wx, int wy,
+                                                                          int accumulate, const float* __restrict__ f,
+                                                                          const float* __restrict__ lin,
+                                                                          const double* __restrict__ gout,
+                                                                          float* __restrict__ g) {
+    constexpr int PER = C / 32;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const float coef = (float)((__ldg(gout + layer) + __ldg(gout + LP_LAYERS)) * 2.0 / pixels);
+    float w[PER];
+#pragma unroll
+    for (int i = 0; i < PER; ++i) w[i] = __ldg(lin + lane + 32 * i);
+    for (int j = 0; j < LP_TAP_PIX; ++j) {
+        const int p = (blockIdx.x * LP_TAP_WARPS + warp) * LP_TAP_PIX + j;
+        if (p >= P) break;
+        const float* fx = f + (size_t)p * C;
+        const float* fy = f + ((size_t)P + p) * C;
+        float xv[PER], yv[PER], u[PER], sx = 0.f, sy = 0.f;
+#pragma unroll
+        for (int i = 0; i < PER; ++i) {
+            xv[i] = __ldg(fx + lane + 32 * i);
+            yv[i] = __ldg(fy + lane + 32 * i);
+            sx = fmaf(xv[i], xv[i], sx);
+            sy = fmaf(yv[i], yv[i], sy);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            sx += __shfl_xor_sync(0xffffffffu, sx, o);
+            sy += __shfl_xor_sync(0xffffffffu, sy, o);
+        }
+        const float ax = sqrtf(sx), ay = sqrtf(sy), nx = ax + 1e-10f, ny = ay + 1e-10f;
+#pragma unroll
+        for (int i = 0; i < PER; ++i) u[i] = coef * w[i] * (__fdiv_rn(xv[i], nx) - __fdiv_rn(yv[i], ny));
+#pragma unroll
+        for (int side = 0; side < 2; ++side) {
+            if (side == 0 ? !wx : !wy) continue;
+            const float* fv = side == 0 ? xv : yv;
+            const float norm = side == 0 ? ax : ay, D = side == 0 ? nx : ny, sgn = side == 0 ? 1.f : -1.f;
+            float dot = 0.f;
+#pragma unroll
+            for (int i = 0; i < PER; ++i) dot = fmaf(u[i], fv[i], dot);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+            // (u.f) / |f| / D / D one division at a time: |f| D^2 underflows for tiny non-zero features
+            const float k = norm > 0.f ? __fdiv_rn(__fdiv_rn(__fdiv_rn(dot, norm), D), D) : 0.f;
+            float* gr = g + ((size_t)(side == 0 ? 0 : (wx ? P : 0)) + p) * C;
+#pragma unroll
+            for (int i = 0; i < PER; ++i) {
+                const float d = sgn * (__fdiv_rn(u[i], D) - fv[i] * k);
+                const float v = accumulate ? gr[lane + 32 * i] + d : d;
+                gr[lane + 32 * i] = fv[i] > 0.f ? v : 0.f;
+            }
+        }
+    }
+}
+
+// Max-pool 3/2 backward as a gather over the conv output grid [NB][H][W][C] (float4 units): each element sums dout
+// over the (at most 2 x 2) windows containing it in which it is the argmax, recomputed from the saved conv output
+// `in` with torch's rule (the first maximum in row-major order wins ties).  No atomics.
+__global__ void __launch_bounds__(256) lpips_maxpool_bwd_kernel(int total4, int C4, int H, int W, int Ho, int Wo,
+                                                                const float4* __restrict__ in,
+                                                                const float4* __restrict__ dout,
+                                                                float4* __restrict__ din) {
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < total4; e += gridDim.x * blockDim.x) {
+        const int c = e % C4;
+        int r = e / C4;
+        const int ix = r % W;
+        r /= W;
+        const int iy = r % H, n = r / H;
+        const int oy0 = iy < 2 ? 0 : (iy - 1) / 2, oy1 = min(iy / 2, Ho - 1);
+        const int ox0 = ix < 2 ? 0 : (ix - 1) / 2, ox1 = min(ix / 2, Wo - 1);
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int oy = oy0; oy <= oy1; ++oy)
+            for (int ox = ox0; ox <= ox1; ++ox) {
+                const float4* p = in + (((size_t)n * H + 2 * oy) * W + 2 * ox) * C4 + c;
+                float4 m = __ldg(p);
+                int4 am = make_int4(0, 0, 0, 0);
+#pragma unroll
+                for (int t = 1; t < 9; ++t) {
+                    const float4 q = __ldg(p + ((size_t)(t / 3) * W + t % 3) * C4);
+                    if (q.x > m.x) { m.x = q.x; am.x = t; }
+                    if (q.y > m.y) { m.y = q.y; am.y = t; }
+                    if (q.z > m.z) { m.z = q.z; am.z = t; }
+                    if (q.w > m.w) { m.w = q.w; am.w = t; }
+                }
+                const int self = (iy - 2 * oy) * 3 + (ix - 2 * ox);
+                const float4 d = __ldg(dout + (((size_t)n * Ho + oy) * Wo + ox) * C4 + c);
+                if (am.x == self) acc.x += d.x;
+                if (am.y == self) acc.y += d.y;
+                if (am.z == self) acc.z += d.z;
+                if (am.w == self) acc.w += d.w;
+            }
+        din[e] = acc;
+    }
+}
+
+// Layer-1 dgrad (11x11, stride 4, pad 2, Cin 3) on the CUDA cores in fp32: three output channels would fill a
+// 64-wide tensor-core tile to 5%.  dz[c][iy][ix] = sum over the <= 3 x 3 (ky, kx) with ky = iy + 2 (mod 4), oy =
+// (iy + 2 - ky) / 4, and likewise in x, of sum_co dY[oy][ox][co] w[co][c][ky][kx]; the image gradient is dz / scale,
+// a true division like the forward's z-score.  Each block takes one phase (iy mod 4, ix mod 4) of one image, so its
+// threads share the same taps, whose weights it stages in shared memory; a 32 x 8 block covers 128 x 32 pixels.
+constexpr int LP_D0_TX = 32, LP_D0_TY = 8;
+struct LpDgrad0Args {
+    const float* dy;       // [NB][Ho][Wo][64], the gradient of conv 1's pre-ReLU output
+    const float* w;        // [64][3][11][11]
+    float* first;          // images 0..N-1 of dy: [N][3][H][W]
+    float* second;         // images N..NB-1 (NB = 2N)
+    int N, H, W, Ho, Wo, tiles_x, tiles_y;
+};
+__global__ void __launch_bounds__(LP_D0_TX * LP_D0_TY) lpips_dgrad0_kernel(const __grid_constant__ LpDgrad0Args a) {
+    constexpr int KS = 11, S = 4, PAD = 2, CO = 64;
+    __shared__ float4 s_w[3][3][CO];
+    int b = blockIdx.x;
+    const int tx = b % a.tiles_x; b /= a.tiles_x;
+    const int ty = b % a.tiles_y; b /= a.tiles_y;
+    const int phase = b % (S * S), n = b / (S * S);
+    const int py = phase / S, px = phase % S;
+    const int ry = (py + PAD) % S, rx = (px + PAD) % S;   // ky = ry + 4 i, kx = rx + 4 j
+    for (int e = threadIdx.y * LP_D0_TX + threadIdx.x; e < 9 * CO; e += LP_D0_TX * LP_D0_TY) {
+        const int co = e % CO, t = e / CO, ky = ry + S * (t / 3), kx = rx + S * (t % 3);
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (ky < KS && kx < KS) {
+            const float* wp = a.w + ((size_t)co * 3 * KS + ky) * KS + kx;
+            v = make_float4(__ldg(wp), __ldg(wp + KS * KS), __ldg(wp + 2 * KS * KS), 0.f);
+        }
+        s_w[t / 3][t % 3][co] = v;
+    }
+    __syncthreads();
+    const int iy = S * (ty * LP_D0_TY + threadIdx.y) + py, ix = S * (tx * LP_D0_TX + threadIdx.x) + px;
+    if (iy >= a.H || ix >= a.W) return;
+    float ax = 0.f, ay = 0.f, az = 0.f;
+    for (int i = 0; i < 3; ++i) {
+        const int ky = ry + S * i, ny = iy + PAD - ky;
+        if (ky >= KS || ny < 0) continue;
+        const int oy = ny / S;
+        if (oy >= a.Ho) continue;
+        for (int j = 0; j < 3; ++j) {
+            const int kx = rx + S * j, nx = ix + PAD - kx;
+            if (kx >= KS || nx < 0) continue;
+            const int ox = nx / S;
+            if (ox >= a.Wo) continue;
+            const float4* g = reinterpret_cast<const float4*>(a.dy + (((size_t)n * a.Ho + oy) * a.Wo + ox) * CO);
+#pragma unroll 4
+            for (int c4 = 0; c4 < CO / 4; ++c4) {
+                const float4 d = __ldg(g + c4);
+                const float4 w0 = s_w[i][j][4 * c4], w1 = s_w[i][j][4 * c4 + 1];
+                const float4 w2 = s_w[i][j][4 * c4 + 2], w3 = s_w[i][j][4 * c4 + 3];
+                ax = fmaf(d.x, w0.x, ax); ay = fmaf(d.x, w0.y, ay); az = fmaf(d.x, w0.z, az);
+                ax = fmaf(d.y, w1.x, ax); ay = fmaf(d.y, w1.y, ay); az = fmaf(d.y, w1.z, az);
+                ax = fmaf(d.z, w2.x, ax); ay = fmaf(d.z, w2.y, ay); az = fmaf(d.z, w2.z, az);
+                ax = fmaf(d.w, w3.x, ax); ay = fmaf(d.w, w3.y, ay); az = fmaf(d.w, w3.z, az);
+            }
+        }
+    }
+    float* out = n < a.N ? a.first + (size_t)n * 3 * a.H * a.W : a.second + (size_t)(n - a.N) * 3 * a.H * a.W;
+    const size_t hw = (size_t)a.H * a.W, o = (size_t)iy * a.W + ix;
+    // the float32 scale of networks.py:44 (lpips_conv_kernel<0>'s gather)
+    out[o] = __fdiv_rn(ax, .458f);
+    out[hw + o] = __fdiv_rn(ay, .448f);
+    out[2 * hw + o] = __fdiv_rn(az, .450f);
 }
 
 }  // namespace s3g

@@ -6,6 +6,12 @@ the fifth ReLU, channel-normalised taps, the v0.1 ``lin`` weights, layer means s
 the images).  The convolutions run as implicit GEMMs on the tensor cores in 3xTF32 (s3g_lpips_alex, csrc/lpips.cuh);
 the result is a float32 [1,1,1,1] tensor on the inputs' device, computed without host synchronisation.
 
+Like the reference's module, the result is differentiable with respect to x and y (the weights are frozen), so it can
+be a training loss.  When grad is enabled and x or y requires grad, the call keeps the forward's activations (about
+0.24 GB per 1920x1280 pair) until the backward, s3g_lpips_alex_backward: ReLU masks, max-pool argmaxes and taps from
+those activations, the convolutions' input gradients as 3xTF32 implicit GEMMs on the tensor cores (conv 1's on the CUDA
+cores).  Its weight layout is made on the first backward on a device.  Any other call keeps nothing.
+
 Weights are never downloaded.  By default they are read from the files the reference's run leaves in the torch hub
 cache, ``torch.hub.get_dir()/checkpoints``: ``alexnet-owt-7be5be79.pth`` (torchvision's AlexNet state dict; only
 ``features.{0,3,6,8,10}`` is used) and ``alex.pth`` (LPIPS v0.1 lin layers, ``lin{i}.model.1.weight``).
@@ -21,6 +27,7 @@ import ctypes as C
 import os
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 
@@ -85,6 +92,7 @@ class LPIPS:
         self._conv_b = [get(features_sd, f"features.{i}.bias", s[:1]) for i, s in zip(FEATURE_INDICES, CONV_SHAPES)]
         self._lin = [get(lin_sd, f"lin{i}.model.1.weight", (1, c, 1, 1)) for i, c in enumerate(CHANNELS)]
         self._prepared = {}                 # device -> (prepared buffer, the device weights it was made from)
+        self._prepared_bwd = {}             # device -> the backward's prepared buffer
 
     def _prepared_on(self, dev: torch.device) -> torch.Tensor:
         """The weights in the kernels' layout on `dev`, made once (pinned host copies, so no host synchronisation)."""
@@ -103,8 +111,39 @@ class LPIPS:
             self._prepared[dev] = (buf, ws)
         return self._prepared[dev][0]
 
+    def _prepared_bwd_on(self, dev: torch.device) -> torch.Tensor:
+        """The backward's weight layout on `dev`, made the first time a backward runs there, from the device weight
+        copies _prepared_on keeps (no host synchronisation)."""
+        if dev not in self._prepared_bwd:
+            lib = _lib.load()
+            ws = self._prepared[dev][1]
+            buf = torch.empty(int(lib.s3g_lpips_alex_backward_prepared_bytes()), dtype=torch.uint8, device=dev)
+            desc = _lib.LpipsAlexWeights()
+            for i in range(5):
+                desc.conv_w[i] = ws[i].data_ptr()
+                desc.conv_b[i] = ws[5 + i].data_ptr()
+                desc.lin_w[i] = ws[10 + i].data_ptr()
+            _lib.check(lib.s3g_lpips_alex_backward_prepare(C.byref(desc), buf.data_ptr(),
+                                                           C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                       "lpips_alex_backward_prepare")
+            self._prepared_bwd[dev] = buf
+        return self._prepared_bwd[dev]
+
+    def _run(self, N: int, H: int, W: int, xf: torch.Tensor, yf: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+        """(out [6], the workspace holding every activation) of one s3g_lpips_alex call on the current device."""
+        lib = _lib.load()
+        dev = xf.device
+        prepared = self._prepared_on(dev)
+        ws = torch.empty(int(lib.s3g_lpips_alex_workspace_bytes(N, H, W)), dtype=torch.uint8, device=dev)
+        out = torch.empty(6, dtype=torch.float64, device=dev)
+        _lib.check(lib.s3g_lpips_alex(N, H, W, xf.data_ptr(), yf.data_ptr(), prepared.data_ptr(), out.data_ptr(),
+                                      ws.data_ptr(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                   "lpips_alex")
+        return out, ws
+
     def terms(self, x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
-        """DEVICE float64 [6]: the five layer terms (each summed over the N pairs), then their sum."""
+        """DEVICE float64 [6]: the five layer terms (each summed over the N pairs), then their sum.  Differentiable
+        with respect to x and y (not the frozen weights) when grad is enabled and either requires grad."""
         if x.dim() not in (3, 4) or tuple(x.shape) != tuple(y.shape):
             raise ValueError(f"x and y must both be [3,H,W] or [N,3,H,W], got {tuple(x.shape)} and {tuple(y.shape)}")
         N, Cn, H, W = (1, *x.shape) if x.dim() == 3 else tuple(x.shape)
@@ -122,17 +161,49 @@ class LPIPS:
             raise ValueError(f"{N} images of {H}x{W} are too large for one LPIPS call (32-bit indices)")
         dev = x.device
         with torch.cuda.device(dev):
-            prepared = self._prepared_on(dev)
             xf, yf = x.float().contiguous(), y.float().contiguous()
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            out = torch.empty(6, dtype=torch.float64, device=dev)
-            _lib.check(lib.s3g_lpips_alex(N, H, W, xf.data_ptr(), yf.data_ptr(), prepared.data_ptr(), out.data_ptr(),
-                                          ws.data_ptr(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-                       "lpips_alex")
+            if torch.is_grad_enabled() and (xf.requires_grad or yf.requires_grad):
+                return _LpipsAlexFunction.apply(xf, yf, self, (N, H, W))
+            out, _ = self._run(N, H, W, xf, yf)
         return out
 
     def __call__(self, x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
         return self.terms(x, y)[5:].to(torch.float32).view(1, 1, 1, 1)
+
+
+class _LpipsAlexFunction(torch.autograd.Function):
+    """terms() with gradients for x and y: the forward keeps its workspace (every activation, about 0.24 GB per
+    1920x1280 pair) until the backward, which reads it in s3g_lpips_alex_backward on the current stream."""
+
+    @staticmethod
+    def forward(ctx, xf, yf, fn, shape):
+        out, ws = fn._run(*shape, xf, yf)
+        ctx.save_for_backward(ws)
+        ctx.fn, ctx.shape, ctx.in_shape = fn, shape, xf.shape
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        (ws,) = ctx.saved_tensors
+        fn, (N, H, W) = ctx.fn, ctx.shape
+        dev = ws.device
+        lib = _lib.load()
+        with torch.cuda.device(dev):
+            prepared, prepared_bwd = fn._prepared_on(dev), fn._prepared_bwd_on(dev)
+            # written as [N,3,H,W]; a [3,H,W] input gets a [3,H,W] gradient
+            gx, gy = (torch.empty(ctx.in_shape, dtype=torch.float32, device=dev) if need else None
+                      for need in ctx.needs_input_grad[:2])
+            g = grad_out.to(dev, torch.float64).contiguous()
+            work = torch.empty(int(lib.s3g_lpips_alex_backward_workspace_bytes(N, H, W)), dtype=torch.uint8,
+                               device=dev)
+            _lib.check(lib.s3g_lpips_alex_backward(N, H, W, prepared.data_ptr(), prepared_bwd.data_ptr(),
+                                                   ws.data_ptr(), g.data_ptr(),
+                                                   None if gx is None else gx.data_ptr(),
+                                                   None if gy is None else gy.data_ptr(), work.data_ptr(),
+                                                   C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                       "lpips_alex_backward")
+        return gx, gy, None, None
 
 
 _cached: dict = {}
