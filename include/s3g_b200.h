@@ -298,6 +298,38 @@ int s3g_lpips_alex_backward(int N, int H, int W, const void* prepared, const voi
                             const void* fwd_workspace, const double* grad_out, float* grad_x, float* grad_y,
                             void* workspace, void* stream);
 
+/* ---- LPIPS v0.1, VGG16 backbone (metrics.py:74 calls lpips(renders[idx], gts[idx], net_type='vgg')) ---------------
+ * The same computation as s3g_lpips_alex on another network (csrc/lpips_vgg.cuh), forward only:
+ *   lpipsPyTorch/modules/networks.py:50-51   the same z-score
+ *   lpipsPyTorch/modules/networks.py:53-63,88-96
+ *                                            torchvision vgg16().features up to relu5_3: 3x3 pad 1 convolutions
+ *                                            3->64, 64->64 | 64->128, 128->128 | 128->256, 256->256 x2 |
+ *                                            256->512, 512->512 x2 | 512->512 x3, each followed by a ReLU, a 2/2
+ *                                            max-pool (floor) between the groups; taps after the last ReLU of each
+ *                                            group (64, 128, 256, 512, 512 channels)
+ *   lpipsPyTorch/modules/utils.py:6-8, lpips.py:30-36   taps, lin weights, layer means and sums as above
+ * 3xTF32 implicit GEMMs with fp32 accumulation, 128-channel tiles where Cout >= 128.
+ *
+ * s3g_lpips_vgg_prepare / s3g_lpips_vgg: as the AlexNet pair, with `prepared` of s3g_lpips_vgg_prepared_bytes()
+ * (about 118 MB) and H, W >= 16 (smaller sides make the fourth max-pool's output empty; torch raises).  out[l] is the
+ * term of tap l (0..4) summed over the N images, out[5] their sum.  No host synchronisation, no atomics: two calls give
+ * bitwise equal results.  Nothing is kept for a backward.
+ * workspace: s3g_lpips_vgg_workspace_bytes(N, H, W) bytes (0 for invalid sizes): two buffers of 2N * H * W * 64 floats
+ * that the layers ping-pong between (x's and y's images walk each layer together) plus the taps' partial sums, 2.52 GB
+ * for one 1920x1280 pair.
+ * S3G_ERR_ARG before any launch: N < 1, a side below 16, a null pointer, an unaligned `prepared`, or 2N * H * W * 64
+ * >= 2^31 (32-bit element indices). */
+typedef struct s3g_lpips_vgg_weights {
+    const float* conv_w[13];  /* features.{0,2,5,7,10,12,14,17,19,21,24,26,28}.weight, [Cout,Cin,3,3] */
+    const float* conv_b[13];  /* the same indices' .bias, [Cout] */
+    const float* lin_w[5];    /* lin{i}.model.1.weight, [1,C,1,1] (C floats) */
+} s3g_lpips_vgg_weights;
+size_t s3g_lpips_vgg_prepared_bytes(void);
+int s3g_lpips_vgg_prepare(const s3g_lpips_vgg_weights* weights, void* prepared, void* stream);
+size_t s3g_lpips_vgg_workspace_bytes(int N, int H, int W);
+int s3g_lpips_vgg(int N, int H, int W, const float* x, const float* y, const void* prepared, double* out,
+                  void* workspace, void* stream);
+
 /* ---- state-buffer introspection (tests / debugging) ---------------------
  * buffer: 0 = geometry, 1 = binning, 2 = image.  Looks up a named field of our
  * layout for the given problem size and returns its byte offset from the

@@ -41,6 +41,11 @@ SIGNATURES = {
     "s3g_lpips_alex_backward_prepare": (_I, [_V, _V, _V]),
     "s3g_lpips_alex_backward_workspace_bytes": (_SZ, [_I, _I, _I]),
     "s3g_lpips_alex_backward": (_I, [_I, _I, _I, _V, _V, _V, _V, _V, _V, _V, _V]),
+    # s3g_lpips_vgg_prepare takes an LpipsVggWeights (below) with ctypes.byref()
+    "s3g_lpips_vgg_prepared_bytes": (_SZ, []),
+    "s3g_lpips_vgg_prepare": (_I, [_V, _V, _V]),
+    "s3g_lpips_vgg_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "s3g_lpips_vgg": (_I, [_I, _I, _I, _V, _V, _V, _V, _V, _V]),
     "s3g_peer_reduce_gather": (_I, [_I, _I, _V, _V, _V, _I64, _I64, _V]),
     "s3g_state_field": (_I, [_I, C.c_char_p, _I64, _I64, _I, _I, C.POINTER(_SZ), C.POINTER(_SZ),
                              C.POINTER(_SZ)]),
@@ -188,3 +193,8 @@ class RowTensor(C.Structure):
 class LpipsAlexWeights(C.Structure):
     """s3g_lpips_alex_weights (include/s3g_b200.h)."""
     _fields_ = [("conv_w", C.c_void_p * 5), ("conv_b", C.c_void_p * 5), ("lin_w", C.c_void_p * 5)]
+
+
+class LpipsVggWeights(C.Structure):
+    """s3g_lpips_vgg_weights (include/s3g_b200.h)."""
+    _fields_ = [("conv_w", C.c_void_p * 13), ("conv_b", C.c_void_p * 13), ("lin_w", C.c_void_p * 5)]

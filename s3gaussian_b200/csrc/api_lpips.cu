@@ -1,10 +1,11 @@
-// api_lpips.cu - extern "C" entry points of LPIPS (AlexNet, v0.1) (include/s3g_b200.h, csrc/lpips.cuh).
+// api_lpips.cu - extern "C" entry points of LPIPS v0.1, AlexNet and VGG16 backbones (include/s3g_b200.h,
+// csrc/lpips.cuh, csrc/lpips_vgg.cuh).
 #include <algorithm>
 #include <cstdint>
 
 #include "api_common.cuh"
 #include "common.cuh"
-#include "lpips.cuh"
+#include "lpips_vgg.cuh"
 
 using namespace s3g;
 
@@ -16,9 +17,9 @@ struct LpPrepared {
     size_t tiles[LP_LAYERS], bias[LP_LAYERS], lin[LP_LAYERS], total;
     LpPrepared() {
         size_t o = 0;
-        for (int l = 0; l < LP_LAYERS; ++l) { tiles[l] = o; o += (size_t)lp_tiles(l) * LP_TILE_FLOATS; }
-        for (int l = 0; l < LP_LAYERS; ++l) { bias[l] = o; o += lp_cout(l); }
-        for (int l = 0; l < LP_LAYERS; ++l) { lin[l] = o; o += lp_cout(l); }
+        for (int l = 0; l < LP_LAYERS; ++l) { tiles[l] = o; o += (size_t)lp_prep_floats<LpAlex>(l); }
+        for (int l = 0; l < LP_LAYERS; ++l) { bias[l] = o; o += LpAlex::cout(l); }
+        for (int l = 0; l < LP_LAYERS; ++l) { lin[l] = o; o += LpAlex::cout(l); }
         total = o;
     }
 };
@@ -36,14 +37,14 @@ struct LpShapes {
         size_t o = 0;
         auto take = [&](int64_t bytes_) { const size_t at = o; o += ((size_t)bytes_ + 255) & ~(size_t)255; return at; };
         for (int l = 0; l < LP_LAYERS; ++l) {
-            h[l] = (ih + 2 * lp_pad(l) - lp_ks(l)) / lp_stride(l) + 1;
-            w[l] = (iw + 2 * lp_pad(l) - lp_ks(l)) / lp_stride(l) + 1;
-            conv_elems[l] = NI * h[l] * w[l] * lp_cout(l);
+            h[l] = (ih + 2 * LpAlex::pad(l) - LpAlex::ks(l)) / LpAlex::stride(l) + 1;
+            w[l] = (iw + 2 * LpAlex::pad(l) - LpAlex::ks(l)) / LpAlex::stride(l) + 1;
+            conv_elems[l] = NI * h[l] * w[l] * LpAlex::cout(l);
             conv_off[l] = take(conv_elems[l] * 4);
             ih = h[l]; iw = w[l];
             if (l < 2) {
                 ph[l] = (ih - 3) / 2 + 1; pw[l] = (iw - 3) / 2 + 1;
-                pool_elems[l] = NI * ph[l] * pw[l] * lp_cout(l);
+                pool_elems[l] = NI * ph[l] * pw[l] * LpAlex::cout(l);
                 pool_off[l] = take(pool_elems[l] * 4);
                 ih = ph[l]; iw = pw[l];
             }
@@ -70,9 +71,9 @@ struct LpPreparedBwd {
     size_t w0, tiles[LP_LAYERS], total;
     LpPreparedBwd() {
         size_t o = 0;
-        w0 = o; o += (size_t)lp_cout(0) * lp_k(0);
+        w0 = o; o += (size_t)LpAlex::cout(0) * lp_k<LpAlex>(0);
         tiles[0] = 0;
-        for (int l = 1; l < LP_LAYERS; ++l) { tiles[l] = o; o += (size_t)lp_tiles(l) * LP_TILE_FLOATS; }
+        for (int l = 1; l < LP_LAYERS; ++l) { tiles[l] = o; o += (size_t)lp_prep_floats<LpAlex>(l); }
         total = o;
     }
 };
@@ -92,10 +93,10 @@ struct LpBwdShapes {
 
 template <int L>
 int launch_dgrad(const LpConvArgs& a, cudaStream_t stream) {
-    S3G_CUDA(cudaFuncSetAttribute(lpips_dgrad_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, LP_SMEM_BYTES),
+    S3G_CUDA(cudaFuncSetAttribute(lpips_dgrad_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, lp_smem_bytes(LpAlex::bn(L))),
              "lpips dgrad smem attribute");
-    const dim3 grid((unsigned)div_up64(a.M, LP_BM), lp_cin(L) / LP_BN);
-    lpips_dgrad_kernel<L><<<grid, LP_THREADS, LP_SMEM_BYTES, stream>>>(a);
+    const dim3 grid((unsigned)div_up64(a.M, LP_BM), LpAlex::cin(L) / LpAlex::bn(L));
+    lpips_dgrad_kernel<L><<<grid, LP_THREADS, lp_smem_bytes(LpAlex::bn(L)), stream>>>(a);
     S3G_CUDA(cudaGetLastError(), "lpips dgrad launch");
     return S3G_OK;
 }
@@ -112,7 +113,7 @@ int launch_tap_bwd(int P, int layer, double pixels, int wx, int wy, int accumula
 
 int tap_bwd(int l, int P, double pixels, int wx, int wy, int accumulate, const float* f, const float* lin,
             const double* gout, float* g, cudaStream_t stream) {
-    switch (lp_cout(l)) {
+    switch (LpAlex::cout(l)) {
         case 64: return launch_tap_bwd<64>(P, l, pixels, wx, wy, accumulate, f, lin, gout, g, stream);
         case 192: return launch_tap_bwd<192>(P, l, pixels, wx, wy, accumulate, f, lin, gout, g, stream);
         case 384: return launch_tap_bwd<384>(P, l, pixels, wx, wy, accumulate, f, lin, gout, g, stream);
@@ -124,10 +125,10 @@ bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p
 
 template <int L>
 int launch_conv(const LpConvArgs& a, cudaStream_t stream) {
-    S3G_CUDA(cudaFuncSetAttribute(lpips_conv_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, LP_SMEM_BYTES),
+    S3G_CUDA(cudaFuncSetAttribute(lpips_conv_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, lp_smem_bytes(LpAlex::bn(L))),
              "lpips conv smem attribute");
-    const dim3 grid((unsigned)div_up64(a.M, LP_BM), lp_cout(L) / LP_BN);
-    lpips_conv_kernel<L><<<grid, LP_THREADS, LP_SMEM_BYTES, stream>>>(a);
+    const dim3 grid((unsigned)div_up64(a.M, LP_BM), LpAlex::cout(L) / LpAlex::bn(L));
+    lpips_conv_kernel<L><<<grid, LP_THREADS, lp_smem_bytes(LpAlex::bn(L)), stream>>>(a);
     S3G_CUDA(cudaGetLastError(), "lpips conv launch");
     return S3G_OK;
 }
@@ -137,6 +138,83 @@ int launch_tap(int P, int64_t blocks, const float* f, const float* lin, double* 
     lpips_tap_kernel<C><<<(unsigned)blocks, 32 * LP_TAP_WARPS, 0, stream>>>(P, f, lin, partial);
     S3G_CUDA(cudaGetLastError(), "lpips tap launch");
     return S3G_OK;
+}
+
+// the tap of a feature map with C channels (AlexNet's and VGG16's tap widths)
+int tap_fwd(int C, int P, int64_t blocks, const float* f, const float* lin, double* partial, cudaStream_t stream) {
+    switch (C) {
+        case 64: return launch_tap<64>(P, blocks, f, lin, partial, stream);
+        case 128: return launch_tap<128>(P, blocks, f, lin, partial, stream);
+        case 192: return launch_tap<192>(P, blocks, f, lin, partial, stream);
+        case 256: return launch_tap<256>(P, blocks, f, lin, partial, stream);
+        case 384: return launch_tap<384>(P, blocks, f, lin, partial, stream);
+        case 512: return launch_tap<512>(P, blocks, f, lin, partial, stream);
+        default: return fail(S3G_ERR_ARG, "lpips tap: unsupported channel count");
+    }
+}
+
+// ---- VGG16 (lpips_vgg.cuh) -----------------------------------------------------------------------------------------
+constexpr int VGG_MIN_SIDE = 16;   // below it the fourth max-pool's output is empty
+
+// float offsets inside the VGG prepared buffer: the thirteen convolutions' weight tiles, every bias, the five lin weights
+struct LpVggPrepared {
+    size_t tiles[LpVgg::CONVS], bias[LpVgg::CONVS], lin[LP_LAYERS], total;
+    LpVggPrepared() {
+        size_t o = 0;
+        for (int l = 0; l < LpVgg::CONVS; ++l) { tiles[l] = o; o += (size_t)lp_prep_floats<LpVgg>(l); }
+        for (int l = 0; l < LpVgg::CONVS; ++l) { bias[l] = o; o += LpVgg::cout(l); }
+        for (int g = 0; g < LP_LAYERS; ++g) { lin[g] = o; o += LpVgg::cout(LpVgg::last(g)); }
+        total = o;
+    }
+};
+
+// One call's workspace: two activation buffers the layers ping-pong between, each as large as a group-1 convolution's
+// output (the largest tensor: every max-pool quarters the pixels and the channels at most double), and the taps'
+// partial sums.  Group g works on an (H >> g) x (W >> g) grid.
+struct LpVggShapes {
+    int64_t h[LP_LAYERS], w[LP_LAYERS], act_elems, tap_blocks[LP_LAYERS];
+    size_t act_off[2], part_off[LP_LAYERS], bytes;
+    LpVggShapes(int N, int H, int W) {
+        size_t o = 0;
+        auto take = [&](int64_t bytes_) { const size_t at = o; o += ((size_t)bytes_ + 255) & ~(size_t)255; return at; };
+        act_elems = 2 * (int64_t)N * H * W * LpVgg::cout(0);
+        for (int i = 0; i < 2; ++i) act_off[i] = take(act_elems * 4);
+        for (int g = 0; g < LP_LAYERS; ++g) {
+            h[g] = H >> g; w[g] = W >> g;
+            tap_blocks[g] = div_up64((int64_t)N * h[g] * w[g], LP_TAP_WARPS * LP_TAP_PIX);
+            part_off[g] = take(tap_blocks[g] * 8);
+        }
+        bytes = o + 256;   // + alignment of the base
+    }
+};
+
+bool vgg_args_ok(int N, int H, int W) {
+    return N >= 1 && H >= VGG_MIN_SIDE && W >= VGG_MIN_SIDE && 2 * (int64_t)N * H * W * LpVgg::cout(0) < INT32_MAX;
+}
+
+template <int L>
+int launch_vgg_conv(const LpConvArgs& a, cudaStream_t stream) {
+    constexpr int BN = LpVgg::bn(L);
+    S3G_CUDA(cudaFuncSetAttribute(lpips_vgg_conv_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, lp_smem_bytes(BN)),
+             "lpips vgg conv smem attribute");
+    const dim3 grid((unsigned)div_up64(a.M, LP_BM), LpVgg::cout(L) / BN);
+    lpips_vgg_conv_kernel<L><<<grid, LP_THREADS, lp_smem_bytes(BN), stream>>>(a);
+    S3G_CUDA(cudaGetLastError(), "lpips vgg conv launch");
+    return S3G_OK;
+}
+
+// convolutions of one shape share a kernel: 5, 6 are 256 -> 256, 8..12 are 512 -> 512
+int vgg_conv(int l, const LpConvArgs& a, cudaStream_t stream) {
+    switch (l) {
+        case 0: return launch_vgg_conv<0>(a, stream);
+        case 1: return launch_vgg_conv<1>(a, stream);
+        case 2: return launch_vgg_conv<2>(a, stream);
+        case 3: return launch_vgg_conv<3>(a, stream);
+        case 4: return launch_vgg_conv<4>(a, stream);
+        case 5: case 6: return launch_vgg_conv<5>(a, stream);
+        case 7: return launch_vgg_conv<7>(a, stream);
+        default: return launch_vgg_conv<8>(a, stream);
+    }
 }
 }  // namespace
 
@@ -154,16 +232,16 @@ int s3g_lpips_alex_prepare(const s3g_lpips_alex_weights* wts, void* prepared, vo
         return fail(S3G_ERR_ARG, "lpips_alex_prepare: prepared must be 16-byte aligned");
     const LpPrepared lay;
     float* dst = static_cast<float*>(prepared);
-    LpPrepArgs p;
+    LpPrepArgs<LpAlex> p;
     for (int l = 0; l < LP_LAYERS; ++l) {
         p.w[l] = wts->conv_w[l];
         p.dst[l] = dst + lay.tiles[l];
-        S3G_CUDA(cudaMemcpyAsync(dst + lay.bias[l], wts->conv_b[l], lp_cout(l) * sizeof(float), cudaMemcpyDeviceToDevice,
+        S3G_CUDA(cudaMemcpyAsync(dst + lay.bias[l], wts->conv_b[l], LpAlex::cout(l) * sizeof(float), cudaMemcpyDeviceToDevice,
                                  stream), "lpips_alex_prepare bias copy");
-        S3G_CUDA(cudaMemcpyAsync(dst + lay.lin[l], wts->lin_w[l], lp_cout(l) * sizeof(float), cudaMemcpyDeviceToDevice,
+        S3G_CUDA(cudaMemcpyAsync(dst + lay.lin[l], wts->lin_w[l], LpAlex::cout(l) * sizeof(float), cudaMemcpyDeviceToDevice,
                                  stream), "lpips_alex_prepare lin copy");
     }
-    lpips_prep_kernel<<<dim3(256, LP_LAYERS), 256, 0, stream>>>(p);
+    lpips_prep_kernel<LpAlex><<<dim3(256, LP_LAYERS), 256, 0, stream>>>(p);
     S3G_CUDA(cudaGetLastError(), "lpips_prep launch");
     return S3G_OK;
 }
@@ -209,7 +287,7 @@ int s3g_lpips_alex(int N, int H, int W, const float* x, const float* y, const vo
         if (rc != S3G_OK) return rc;
         in = a.out; ih = a.Ho; iw = a.Wo;
         if (l < 2) {
-            const int C4 = lp_cout(l) / 4;
+            const int C4 = LpAlex::cout(l) / 4;
             const int total4 = (int)(s.pool_elems[l] / 4);
             const int grid = (int)std::min<int64_t>(div_up64(total4, 256), (int64_t)device_sm_count() * 16);
             float* po = buf(s.pool_off[l]);
@@ -225,13 +303,7 @@ int s3g_lpips_alex(int N, int H, int W, const float* x, const float* y, const vo
         const float* f = buf(s.conv_off[l]);
         const float* lin = wp + lay.lin[l];
         double* part = reinterpret_cast<double*>(base + s.part_off[l]);
-        int rc = S3G_OK;
-        switch (lp_cout(l)) {
-            case 64: rc = launch_tap<64>(P, s.tap_blocks[l], f, lin, part, stream); break;
-            case 192: rc = launch_tap<192>(P, s.tap_blocks[l], f, lin, part, stream); break;
-            case 384: rc = launch_tap<384>(P, s.tap_blocks[l], f, lin, part, stream); break;
-            default: rc = launch_tap<256>(P, s.tap_blocks[l], f, lin, part, stream); break;
-        }
+        const int rc = tap_fwd(LpAlex::cout(l), P, s.tap_blocks[l], f, lin, part, stream);
         if (rc != S3G_OK) return rc;
         r.partial[l] = part;
         r.blocks[l] = (int)s.tap_blocks[l];
@@ -254,9 +326,9 @@ int s3g_lpips_alex_backward_prepare(const s3g_lpips_alex_weights* wts, void* pre
         return fail(S3G_ERR_ARG, "lpips_alex_backward_prepare: prepared_bwd must be 16-byte aligned");
     const LpPreparedBwd lay;
     float* dst = static_cast<float*>(prepared_bwd);
-    S3G_CUDA(cudaMemcpyAsync(dst + lay.w0, wts->conv_w[0], (size_t)lp_cout(0) * lp_k(0) * sizeof(float),
+    S3G_CUDA(cudaMemcpyAsync(dst + lay.w0, wts->conv_w[0], (size_t)LpAlex::cout(0) * lp_k<LpAlex>(0) * sizeof(float),
                              cudaMemcpyDeviceToDevice, stream), "lpips_alex_backward_prepare conv 1 copy");
-    LpPrepArgs p{};
+    LpPrepArgs<LpAlex> p{};
     for (int l = 1; l < LP_LAYERS; ++l) {
         p.w[l] = wts->conv_w[l];
         p.dst[l] = dst + lay.tiles[l];
@@ -319,10 +391,10 @@ int s3g_lpips_alex_backward(int N, int H, int W, const void* prepared, const voi
     };
     // gradient at pool p's output (dout) -> gradient at conv p's output (din), argmaxes from the saved conv output
     auto pool = [&](int p, const float* dout, float* din) {
-        const int C4 = lp_cout(p) / 4;
+        const int C4 = LpAlex::cout(p) / 4;
         const int64_t total4 = (int64_t)NB * s.h[p] * s.w[p] * C4;
         const int grid = (int)std::min<int64_t>(div_up64(total4, 256), (int64_t)device_sm_count() * 16);
-        const float* in = saved(s.conv_off[p]) + i0 * s.h[p] * s.w[p] * lp_cout(p);
+        const float* in = saved(s.conv_off[p]) + i0 * s.h[p] * s.w[p] * LpAlex::cout(p);
         lpips_maxpool_bwd_kernel<<<grid, 256, 0, stream>>>((int)total4, C4, (int)s.h[p], (int)s.w[p], (int)s.ph[p],
                                                             (int)s.pw[p], reinterpret_cast<const float4*>(in),
                                                             reinterpret_cast<const float4*>(dout),
@@ -352,6 +424,91 @@ int s3g_lpips_alex_backward(int N, int H, int W, const void* prepared, const voi
     const int64_t blocks = (int64_t)NB * 16 * d.tiles_x * d.tiles_y;
     lpips_dgrad0_kernel<<<(unsigned)blocks, dim3(LP_D0_TX, LP_D0_TY), 0, stream>>>(d);
     S3G_CUDA(cudaGetLastError(), "lpips dgrad0 launch");
+    return S3G_OK;
+}
+
+size_t s3g_lpips_vgg_prepared_bytes(void) { return LpVggPrepared().total * sizeof(float); }
+
+int s3g_lpips_vgg_prepare(const s3g_lpips_vgg_weights* wts, void* prepared, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (!wts || !prepared) return fail(S3G_ERR_ARG, "lpips_vgg_prepare: null weights/prepared");
+    for (int l = 0; l < LpVgg::CONVS; ++l)
+        if (!wts->conv_w[l] || !wts->conv_b[l]) return fail(S3G_ERR_ARG, "lpips_vgg_prepare: null weight pointer");
+    for (int g = 0; g < LP_LAYERS; ++g)
+        if (!wts->lin_w[g]) return fail(S3G_ERR_ARG, "lpips_vgg_prepare: null lin weight pointer");
+    if (!aligned(prepared, 16)) return fail(S3G_ERR_ARG, "lpips_vgg_prepare: prepared must be 16-byte aligned");
+    const LpVggPrepared lay;
+    float* dst = static_cast<float*>(prepared);
+    LpPrepArgs<LpVgg> p;
+    for (int l = 0; l < LpVgg::CONVS; ++l) {
+        p.w[l] = wts->conv_w[l];
+        p.dst[l] = dst + lay.tiles[l];
+        S3G_CUDA(cudaMemcpyAsync(dst + lay.bias[l], wts->conv_b[l], LpVgg::cout(l) * sizeof(float),
+                                 cudaMemcpyDeviceToDevice, stream), "lpips_vgg_prepare bias copy");
+    }
+    for (int g = 0; g < LP_LAYERS; ++g)
+        S3G_CUDA(cudaMemcpyAsync(dst + lay.lin[g], wts->lin_w[g], LpVgg::cout(LpVgg::last(g)) * sizeof(float),
+                                 cudaMemcpyDeviceToDevice, stream), "lpips_vgg_prepare lin copy");
+    lpips_prep_kernel<LpVgg><<<dim3(256, LpVgg::CONVS), 256, 0, stream>>>(p);
+    S3G_CUDA(cudaGetLastError(), "lpips_prep launch");
+    return S3G_OK;
+}
+
+size_t s3g_lpips_vgg_workspace_bytes(int N, int H, int W) {
+    if (!vgg_args_ok(N, H, W)) return 0;
+    return LpVggShapes(N, H, W).bytes;
+}
+
+int s3g_lpips_vgg(int N, int H, int W, const float* x, const float* y, const void* prepared, double* out,
+                  void* workspace, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (N < 1) return fail(S3G_ERR_ARG, "lpips_vgg: N >= 1 images expected");
+    if (H < VGG_MIN_SIDE || W < VGG_MIN_SIDE)
+        return fail(S3G_ERR_ARG, "lpips_vgg: image sides must be >= 16 (VGG16's fourth max-pool)");
+    if (!vgg_args_ok(N, H, W)) return fail(S3G_ERR_ARG, "lpips_vgg: images too large for 32-bit indices");
+    if (!x || !y || !prepared || !out || !workspace) return fail(S3G_ERR_ARG, "lpips_vgg: null x/y/prepared/out/workspace");
+    if (!aligned(prepared, 16)) return fail(S3G_ERR_ARG, "lpips_vgg: unaligned prepared");
+    const LpVggShapes s(N, H, W);
+    const LpVggPrepared lay;
+    const float* wp = static_cast<const float*>(prepared);
+    char* base = reinterpret_cast<char*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+    float* act[2] = {reinterpret_cast<float*>(base + s.act_off[0]), reinterpret_cast<float*>(base + s.act_off[1])};
+
+    // every kernel reads one activation buffer and writes the other
+    LpReduceArgs r;
+    const float* in = nullptr;
+    int o = 0, g = 0;
+    for (int l = 0; l < LpVgg::CONVS; ++l) {
+        const int gh = (int)s.h[g], gw = (int)s.w[g];
+        LpConvArgs a;
+        a.in = in; a.x = x; a.y = y; a.N = N; a.H = a.Ho = gh; a.W = a.Wo = gw;
+        a.M = 2 * N * gh * gw;
+        a.wprep = wp + lay.tiles[l];
+        a.bias = wp + lay.bias[l];
+        a.out = act[o];
+        int rc = vgg_conv(l, a, stream);
+        if (rc != S3G_OK) return rc;
+        in = a.out; o ^= 1;
+        if (l != LpVgg::last(g)) continue;
+        const int C = LpVgg::cout(l);
+        double* part = reinterpret_cast<double*>(base + s.part_off[g]);
+        rc = tap_fwd(C, N * gh * gw, s.tap_blocks[g], in, wp + lay.lin[g], part, stream);
+        if (rc != S3G_OK) return rc;
+        r.partial[g] = part;
+        r.blocks[g] = (int)s.tap_blocks[g];
+        r.pixels[g] = (double)(s.h[g] * s.w[g]);
+        if (++g == LP_LAYERS) break;
+        const int ph = (int)s.h[g], pw = (int)s.w[g];
+        const int total4 = 2 * N * ph * pw * (C / 4);
+        const int grid = (int)std::min<int64_t>(div_up64(total4, 256), (int64_t)device_sm_count() * 16);
+        lpips_maxpool2_kernel<<<grid, 256, 0, stream>>>(total4, C / 4, gh, gw, ph, pw, reinterpret_cast<const float4*>(in),
+                                                        reinterpret_cast<float4*>(act[o]));
+        S3G_CUDA(cudaGetLastError(), "lpips vgg maxpool launch");
+        in = act[o]; o ^= 1;
+    }
+    r.out = out;
+    lpips_reduce_kernel<<<1, 256, 0, stream>>>(r);
+    S3G_CUDA(cudaGetLastError(), "lpips reduce launch");
     return S3G_OK;
 }
 

@@ -19,6 +19,8 @@
 // Taps: one warp per pixel pair normalises both feature vectors over channels, weighs the squared difference with
 // the lin weights and sums it; blocks write double partials, and one fixed-order double reduction writes each
 // layer's mean over its grid (summed over the images) and the total.  No atomics: two calls are bitwise equal.
+// The weight preparation and the convolution tile take the backbone as a table (LpAlex here, LpVgg in lpips_vgg.cuh);
+// the tap and reduction kernels are the same for every backbone.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -27,26 +29,34 @@
 
 namespace s3g {
 
-constexpr int LP_LAYERS = 5;
-constexpr int LP_BM = 128, LP_BN = 64, LP_BK = 32;
+constexpr int LP_LAYERS = 5;                             // taps (every LPIPS backbone here has five)
+constexpr int LP_BM = 128, LP_BK = 32;
 constexpr int LP_THREADS = 128;
 constexpr int LP_A_FLOATS = LP_BM * LP_BK;               // one operand part (hi or lo) of A
-constexpr int LP_B_FLOATS = LP_BN * LP_BK;
-constexpr int LP_TILE_FLOATS = 2 * LP_B_FLOATS;          // one prepared weight tile: hi | lo
-constexpr int LP_STAGE_FLOATS = 2 * LP_A_FLOATS + LP_TILE_FLOATS;
-constexpr int LP_SMEM_BYTES = 2 * LP_STAGE_FLOATS * 4;   // 96 KB: two stages, two CTAs per SM
+// BN = output channels of a CTA's tile, chosen per convolution by the network's table
+__host__ __device__ constexpr int lp_tile_floats(int BN) { return 2 * BN * LP_BK; }   // a prepared weight tile: hi | lo
+__host__ __device__ constexpr int lp_stage_floats(int BN) { return 2 * LP_A_FLOATS + lp_tile_floats(BN); }
+// two stages: 96 KB at BN = 64 (two CTAs per SM), 128 KB at BN = 128 (one)
+__host__ __device__ constexpr int lp_smem_bytes(int BN) { return 2 * lp_stage_floats(BN) * 4; }
 constexpr int LP_TAP_WARPS = 8, LP_TAP_PIX = 8;          // tap kernel: 8 warps x 8 pixels per block
 
-// AlexNet `features` convolutions 0, 3, 6, 8, 10
-__host__ __device__ constexpr int lp_cin(int l) { return l == 0 ? 3 : l == 1 ? 64 : l == 2 ? 192 : l == 3 ? 384 : 256; }
-__host__ __device__ constexpr int lp_cout(int l) { return l == 0 ? 64 : l == 1 ? 192 : l == 2 ? 384 : 256; }
-__host__ __device__ constexpr int lp_ks(int l) { return l == 0 ? 11 : l == 1 ? 5 : 3; }
-__host__ __device__ constexpr int lp_stride(int l) { return l == 0 ? 4 : 1; }
-__host__ __device__ constexpr int lp_pad(int l) { return l <= 1 ? 2 : 1; }
+// A backbone is a table of its convolutions, taken as a template argument by the weight preparation and the
+// convolution tile: input and output channels, kernel size, stride, padding and the tile's BN of convolution l.
+// AlexNet: `features` convolutions 0, 3, 6, 8, 10 (VGG16: lpips_vgg.cuh)
+struct LpAlex {
+    static constexpr int CONVS = 5;
+    __host__ __device__ static constexpr int cin(int l) { return l == 0 ? 3 : l == 1 ? 64 : l == 2 ? 192 : l == 3 ? 384 : 256; }
+    __host__ __device__ static constexpr int cout(int l) { return l == 0 ? 64 : l == 1 ? 192 : l == 2 ? 384 : 256; }
+    __host__ __device__ static constexpr int ks(int l) { return l == 0 ? 11 : l == 1 ? 5 : 3; }
+    __host__ __device__ static constexpr int stride(int l) { return l == 0 ? 4 : 1; }
+    __host__ __device__ static constexpr int pad(int l) { return l <= 1 ? 2 : 1; }
+    __host__ __device__ static constexpr int bn(int) { return 64; }
+};
 
-__host__ __device__ constexpr int lp_k(int l) { return lp_ks(l) * lp_ks(l) * lp_cin(l); }
-__host__ __device__ constexpr int lp_kpad(int l) { return (lp_k(l) + LP_BK - 1) / LP_BK * LP_BK; }
-__host__ __device__ constexpr int lp_tiles(int l) { return (lp_cout(l) / LP_BN) * (lp_kpad(l) / LP_BK); }
+template <class Net> __host__ __device__ constexpr int lp_k(int l) { return Net::ks(l) * Net::ks(l) * Net::cin(l); }
+template <class Net> __host__ __device__ constexpr int lp_kpad(int l) { return (lp_k<Net>(l) + LP_BK - 1) / LP_BK * LP_BK; }
+// floats of convolution l's prepared weights: [Cout / BN][Kpad / 32] tiles
+template <class Net> __host__ __device__ constexpr int lp_prep_floats(int l) { return 2 * Net::cout(l) * lp_kpad<Net>(l); }
 
 // hi = x as is (the tensor core reads its tf32 bits), lo = the truncated remainder (deform.cuh's split_tf32)
 __device__ __forceinline__ void lp_split(float x, uint32_t& hi, uint32_t& lo) {
@@ -55,15 +65,18 @@ __device__ __forceinline__ void lp_split(float x, uint32_t& hi, uint32_t& lo) {
 }
 
 // ---- weight preparation ------------------------------------------------------------------------------------------
+template <class Net>
 struct LpPrepArgs {
-    const float* w[LP_LAYERS];    // [Cout][Cin][k][k], PyTorch layout
-    float* dst[LP_LAYERS];        // lp_tiles(l) prepared tiles
+    const float* w[Net::CONVS];   // [Cout][Cin][k][k], PyTorch layout
+    float* dst[Net::CONVS];       // lp_prep_floats<Net>(l) floats of prepared tiles
 };
 // blockIdx.y = layer; element (co, k) of the padded [Cout][Kpad] matrix in the kernel's K order
-__global__ void __launch_bounds__(256) lpips_prep_kernel(const __grid_constant__ LpPrepArgs p) {
+template <class Net>
+__global__ void __launch_bounds__(256) lpips_prep_kernel(const __grid_constant__ LpPrepArgs<Net> p) {
     const int l = blockIdx.y;
-    const int Cin = lp_cin(l), KS = lp_ks(l), K = lp_k(l), KP = lp_kpad(l), KC = KP / LP_BK;
-    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < lp_cout(l) * KP; e += gridDim.x * blockDim.x) {
+    const int Cin = Net::cin(l), KS = Net::ks(l), K = lp_k<Net>(l), KP = lp_kpad<Net>(l), KC = KP / LP_BK;
+    const int BN = Net::bn(l);
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < Net::cout(l) * KP; e += gridDim.x * blockDim.x) {
         const int co = e / KP, k = e - co * KP;
         float v = 0.f;
         if (k < K) {
@@ -78,20 +91,21 @@ __global__ void __launch_bounds__(256) lpips_prep_kernel(const __grid_constant__
         asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(v));
         const float r = v - __uint_as_float(hi);
         asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(r));
-        float* t = p.dst[l] + (size_t)((co / LP_BN) * KC + k / LP_BK) * LP_TILE_FLOATS;
-        const int ci = umma::canon_idx(co % LP_BN, k % LP_BK, LP_BK);
+        float* t = p.dst[l] + (size_t)((co / BN) * KC + k / LP_BK) * lp_tile_floats(BN);
+        const int ci = umma::canon_idx(co % BN, k % LP_BK, LP_BK);
         t[ci] = __uint_as_float(hi);
-        t[LP_B_FLOATS + ci] = __uint_as_float(lo);
+        t[BN * LP_BK + ci] = __uint_as_float(lo);
     }
 }
 
-// Dgrad weights of convolutions 1..4 (blockIdx.y + 1): B'[ci][k'] with k' = (ky', kx', co) is
+// Dgrad weights of AlexNet's convolutions 1..4 (blockIdx.y + 1): B'[ci][k'] with k' = (ky', kx', co) is
 // w[co][ci][KS-1-ky'][KS-1-kx'], the flipped, transposed kernel, as [Cin / 64][KS*KS*Cout / 32] hi | lo tiles
 // (lpips_dgrad_kernel's K order: 32 consecutive output channels of one tap per chunk).  Layer 0's dgrad runs on the
 // CUDA cores from the PyTorch layout (lpips_dgrad0_kernel).
-__global__ void __launch_bounds__(256) lpips_prep_dgrad_kernel(const __grid_constant__ LpPrepArgs p) {
+__global__ void __launch_bounds__(256) lpips_prep_dgrad_kernel(const __grid_constant__ LpPrepArgs<LpAlex> p) {
+    constexpr int BN = 64;
     const int l = blockIdx.y + 1;
-    const int Cin = lp_cin(l), Cout = lp_cout(l), KS = lp_ks(l), K = KS * KS * Cout, KC = K / LP_BK;
+    const int Cin = LpAlex::cin(l), Cout = LpAlex::cout(l), KS = LpAlex::ks(l), K = KS * KS * Cout, KC = K / LP_BK;
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < Cin * K; e += gridDim.x * blockDim.x) {
         const int ci = e / K, k = e - ci * K;
         const int tap = k / Cout, co = k - tap * Cout;
@@ -101,10 +115,10 @@ __global__ void __launch_bounds__(256) lpips_prep_dgrad_kernel(const __grid_cons
         asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(v));
         const float r = v - __uint_as_float(hi);
         asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(r));
-        float* t = p.dst[l] + (size_t)((ci / LP_BN) * KC + k / LP_BK) * LP_TILE_FLOATS;
-        const int idx = umma::canon_idx(ci % LP_BN, k % LP_BK, LP_BK);
+        float* t = p.dst[l] + (size_t)((ci / BN) * KC + k / LP_BK) * lp_tile_floats(BN);
+        const int idx = umma::canon_idx(ci % BN, k % LP_BK, LP_BK);
         t[idx] = __uint_as_float(hi);
-        t[LP_B_FLOATS + idx] = __uint_as_float(lo);
+        t[BN * LP_BK + idx] = __uint_as_float(lo);
     }
 }
 
@@ -126,15 +140,18 @@ __device__ __forceinline__ void lp_cp16(float* sdst, const float* gsrc) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(umma::smem_u32(sdst)), "l"(gsrc) : "memory");
 }
 
-// One 128 x 64 output tile of convolution L (DG = false), or of the input gradient of convolution L >= 1 (DG = true).
-// The dgrad of a stride-1 "same" convolution is itself one: input dY [NI][H][W][Cout], output dX [NI][H][W][Cin],
-// the same KS and PAD, the kernel flipped and transposed (lpips_prep_dgrad_kernel), no bias and no ReLU.
-template <int L, bool DG>
+// One 128 x BN output tile of Net's convolution L (DG = false), or of the input gradient of convolution L >= 1
+// (DG = true).  The dgrad of a stride-1 "same" convolution is itself one: input dY [NI][H][W][Cout], output dX
+// [NI][H][W][Cin], the same KS and PAD, the kernel flipped and transposed (lpips_prep_dgrad_kernel), no bias and no
+// ReLU.
+template <class Net, int L, bool DG>
 __device__ __forceinline__ void lp_conv_tile(const LpConvArgs& a) {
-    static_assert(!DG || (L > 0 && lp_stride(L) == 1 && 2 * lp_pad(L) == lp_ks(L) - 1), "dgrad: stride-1 same conv");
-    constexpr int Cin = DG ? lp_cout(L) : lp_cin(L), Cout = DG ? lp_cin(L) : lp_cout(L);
-    constexpr int KS = lp_ks(L), S = lp_stride(L), PAD = lp_pad(L);
+    static_assert(!DG || (L > 0 && Net::stride(L) == 1 && 2 * Net::pad(L) == Net::ks(L) - 1), "dgrad: stride-1 same conv");
+    constexpr int Cin = DG ? Net::cout(L) : Net::cin(L), Cout = DG ? Net::cin(L) : Net::cout(L);
+    constexpr int KS = Net::ks(L), S = Net::stride(L), PAD = Net::pad(L);
     constexpr int K = KS * KS * Cin, KC = (K + LP_BK - 1) / LP_BK;
+    constexpr int BN = Net::bn(L), B_FLOATS = BN * LP_BK, TILE_FLOATS = lp_tile_floats(BN), STAGE_FLOATS = lp_stage_floats(BN);
+    static_assert(Cout % BN == 0 && (L == 0 || Cin % LP_BK == 0), "tile shape");
     constexpr uint32_t SBO = (LP_BK / 4) * 128u, MHALF = 8u * SBO;
     extern __shared__ __align__(128) float s_lp[];
     const int tid = threadIdx.x;
@@ -145,7 +162,7 @@ __device__ __forceinline__ void lp_conv_tile(const LpConvArgs& a) {
     const int pix = valid ? m - img * hw : 0;
     const int oy = pix / a.Wo, ox = pix - oy * a.Wo;
     const int iy0 = oy * S - PAD, ix0 = ox * S - PAD;
-    const float* wtiles = a.wprep + (size_t)blockIdx.y * KC * LP_TILE_FLOATS;
+    const float* wtiles = a.wprep + (size_t)blockIdx.y * KC * TILE_FLOATS;
     const float* src = nullptr;     // layer 1: channel 0 of this pixel's image
     if constexpr (!DG && L == 0) src = (img < a.N ? a.x + (size_t)img * 3 * a.H * a.W : a.y + (size_t)(img - a.N) * 3 * a.H * a.W);
 
@@ -181,10 +198,10 @@ __device__ __forceinline__ void lp_conv_tile(const LpConvArgs& a) {
     };
     // A values -> hi/lo operand tiles of `stage`; the chunk's weight tile -> the stage's B by cp.async
     auto stage_in = [&](int c, int stage) {
-        float* st = s_lp + stage * LP_STAGE_FLOATS;
-        const float* wt = wtiles + (size_t)c * LP_TILE_FLOATS;
+        float* st = s_lp + stage * STAGE_FLOATS;
+        const float* wt = wtiles + (size_t)c * TILE_FLOATS;
 #pragma unroll
-        for (int j = 0; j < LP_TILE_FLOATS / 4 / LP_THREADS; ++j)
+        for (int j = 0; j < TILE_FLOATS / 4 / LP_THREADS; ++j)
             lp_cp16(st + 2 * LP_A_FLOATS + 4 * (tid + j * LP_THREADS), wt + 4 * (tid + j * LP_THREADS));
         asm volatile("cp.async.commit_group;" ::: "memory");
 #pragma unroll
@@ -198,16 +215,16 @@ __device__ __forceinline__ void lp_conv_tile(const LpConvArgs& a) {
         }
     };
 
-    float acc[2][LP_BN / 2];
+    float acc[2][BN / 2];
     gather(0);
     stage_in(0, 0);
     for (int c = 0; c < KC; ++c) {
         asm volatile("cp.async.wait_all;" ::: "memory");
         umma::fence_async_smem();
         __syncthreads();
-        const float* st = s_lp + (c & 1) * LP_STAGE_FLOATS;
+        const float* st = s_lp + (c & 1) * STAGE_FLOATS;
         const uint32_t a_hi = umma::smem_u32(st), a_lo = a_hi + LP_A_FLOATS * 4u;
-        const uint32_t b_hi = a_hi + 2u * LP_A_FLOATS * 4u, b_lo = b_hi + LP_B_FLOATS * 4u;
+        const uint32_t b_hi = a_hi + 2u * LP_A_FLOATS * 4u, b_lo = b_hi + B_FLOATS * 4u;
         umma::fence_regs(acc[0]); umma::fence_regs(acc[1]);
         umma::wgmma_fence();
 #pragma unroll
@@ -218,9 +235,9 @@ __device__ __forceinline__ void lp_conv_tile(const LpConvArgs& a) {
             for (int h = 0; h < 2; ++h) {
                 const uint64_t dah = umma::make_smem_desc(a_hi + h * MHALF + off, 128, SBO);
                 const uint64_t dal = umma::make_smem_desc(a_lo + h * MHALF + off, 128, SBO);
-                umma::wgmma_tf32<LP_BN>(acc[h], dal, dbh, c > 0 || k0 > 0);
-                umma::wgmma_tf32<LP_BN>(acc[h], dah, dbl, true);
-                umma::wgmma_tf32<LP_BN>(acc[h], dah, dbh, true);
+                umma::wgmma_tf32<BN>(acc[h], dal, dbh, c > 0 || k0 > 0);
+                umma::wgmma_tf32<BN>(acc[h], dah, dbl, true);
+                umma::wgmma_tf32<BN>(acc[h], dah, dbh, true);
             }
         }
         umma::wgmma_commit();
@@ -233,11 +250,11 @@ __device__ __forceinline__ void lp_conv_tile(const LpConvArgs& a) {
         umma::fence_regs(acc[0]); umma::fence_regs(acc[1]);
     }
     // epilogue: + bias, ReLU (forward only), channels-last store (fragment layout, umma.cuh)
-    const int n0 = blockIdx.y * LP_BN;
+    const int n0 = blockIdx.y * BN;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
 #pragma unroll
-        for (int i = 0; i < LP_BN / 2; i += 2) {
+        for (int i = 0; i < BN / 2; i += 2) {
             const int row = blockIdx.x * LP_BM + 64 * h + umma::frag_row(i);
             const int col = n0 + umma::frag_col(i);
             if (row < a.M) {
@@ -254,13 +271,13 @@ __device__ __forceinline__ void lp_conv_tile(const LpConvArgs& a) {
 
 template <int L>
 __global__ void __launch_bounds__(LP_THREADS, 2) lpips_conv_kernel(const __grid_constant__ LpConvArgs a) {
-    lp_conv_tile<L, false>(a);
+    lp_conv_tile<LpAlex, L, false>(a);
 }
 
 // dX of convolution L (1..4) from dY; a.in = dY, a.out = dX, a.M = images * H * W, a.wprep = the dgrad tiles
 template <int L>
 __global__ void __launch_bounds__(LP_THREADS, 2) lpips_dgrad_kernel(const __grid_constant__ LpConvArgs a) {
-    lp_conv_tile<L, true>(a);
+    lp_conv_tile<LpAlex, L, true>(a);
 }
 
 // ---- max-pool 3/2, no padding, floor mode, channels-last [NI][H][W][C] -> [NI][Ho][Wo][C] ---------------------------

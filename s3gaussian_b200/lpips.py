@@ -49,7 +49,8 @@ def _check_variant(net_type: str, version: str) -> None:
     # lpipsPyTorch/modules/lpips.py:19 asserts the version before get_network (networks.py:12-20) looks at the type
     assert version in ['0.1'], 'v0.1 is only supported now'
     if net_type != 'alex':
-        raise NotImplementedError(f"net_type {net_type!r}: only 'alex' runs on the device ('vgg' and 'squeeze' do not)")
+        raise NotImplementedError(f"net_type {net_type!r}: only 'alex' runs here ('vgg' is s3gaussian_b200.lpips_vgg, "
+                                  f"forward only; 'squeeze' does not run on the device)")
 
 
 def _load(path: str) -> dict:
@@ -57,6 +58,16 @@ def _load(path: str) -> dict:
         raise FileNotFoundError(f"LPIPS weight file not found: {path} (s3gaussian_b200 never downloads weights; "
                                 f"put the file there or pass its path)")
     return torch.load(path, map_location="cpu", weights_only=True)
+
+
+def _get(sd: dict, key: str, shape) -> torch.Tensor:
+    """sd[key] as a contiguous float32 CPU tensor of `shape`."""
+    if key not in sd:
+        raise KeyError(f"LPIPS weights: missing {key!r}")
+    t = torch.as_tensor(sd[key]).detach()
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError(f"LPIPS weights: {key!r} has shape {tuple(t.shape)}, expected {tuple(shape)}")
+    return t.to("cpu", torch.float32).contiguous()
 
 
 class LPIPS:
@@ -81,16 +92,9 @@ class LPIPS:
         return self
 
     def _set_weights(self, features_sd: dict, lin_sd: dict) -> None:
-        def get(sd, key, shape):
-            if key not in sd:
-                raise KeyError(f"LPIPS weights: missing {key!r}")
-            t = torch.as_tensor(sd[key]).detach()
-            if tuple(t.shape) != tuple(shape):
-                raise ValueError(f"LPIPS weights: {key!r} has shape {tuple(t.shape)}, expected {tuple(shape)}")
-            return t.to("cpu", torch.float32).contiguous()
-        self._conv_w = [get(features_sd, f"features.{i}.weight", s) for i, s in zip(FEATURE_INDICES, CONV_SHAPES)]
-        self._conv_b = [get(features_sd, f"features.{i}.bias", s[:1]) for i, s in zip(FEATURE_INDICES, CONV_SHAPES)]
-        self._lin = [get(lin_sd, f"lin{i}.model.1.weight", (1, c, 1, 1)) for i, c in enumerate(CHANNELS)]
+        self._conv_w = [_get(features_sd, f"features.{i}.weight", s) for i, s in zip(FEATURE_INDICES, CONV_SHAPES)]
+        self._conv_b = [_get(features_sd, f"features.{i}.bias", s[:1]) for i, s in zip(FEATURE_INDICES, CONV_SHAPES)]
+        self._lin = [_get(lin_sd, f"lin{i}.model.1.weight", (1, c, 1, 1)) for i, c in enumerate(CHANNELS)]
         self._prepared = {}                 # device -> (prepared buffer, the device weights it was made from)
         self._prepared_bwd = {}             # device -> the backward's prepared buffer
 

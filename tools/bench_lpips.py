@@ -1,4 +1,5 @@
-"""LPIPS (AlexNet, v0.1) per call on the device, four arms, and render_pixels per view with LPIPS (prints one JSON line).
+"""LPIPS (v0.1; AlexNet, or VGG16 with --net vgg) per call on the device, four arms, and render_pixels per view with
+LPIPS (prints one JSON line).
 
   ours         : s3gaussian_b200.lpips.LPIPS - implicit-GEMM convolutions in 3xTF32 (s3g_lpips_alex)
   cudnn_tf32   : the reference's lpipsPyTorch LPIPS module, built once, cuDNN at torch's default (TF32 allowed)
@@ -14,7 +15,13 @@ The render_pixels part times render_pixels per view (fine stage, 12 waymo_ring v
 set up as tools/bench_eval_flow.py does) with lpips_fn set to `ours` and to the cuDNN module (TF32 default),
 alternating, and without lpips_fn for the baseline.
 
-    python tools/bench_lpips.py [--sizes 960x640,1920x1280] [--calls 50] [--rounds 5] [--points 500000] [--views 12]
+--net vgg times s3gaussian_b200.lpips_vgg.LPIPSVGG (s3g_lpips_vgg) against the reference's module built with the
+VGG16 backbone, the same arms and rounds, without the render_pixels part; GFLOP counts the thirteen convolutions.
+`tflop_per_s` counts each multiply-add pair once for every arm: in `ours` the tensor cores execute three times that
+(3xTF32).
+
+    python tools/bench_lpips.py [--net alex] [--sizes 960x640,1920x1280] [--calls 50] [--rounds 5] [--points 500000]
+                                [--views 12]
 """
 from __future__ import annotations
 
@@ -33,6 +40,18 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 CONVS = ((3, 64, 11, 4, 2), (64, 192, 5, 1, 2), (192, 384, 3, 1, 1), (384, 256, 3, 1, 1), (256, 256, 3, 1, 1))
+# VGG16: (Cin, Cout) of the 3x3 / stride 1 / pad 1 convolutions, group by group; a 2x2 max-pool between the groups
+VGG_GROUPS = (((3, 64), (64, 64)), ((64, 128), (128, 128)), ((128, 256), (256, 256), (256, 256)),
+              ((256, 512), (512, 512), (512, 512)), ((512, 512), (512, 512), (512, 512)))
+
+
+def gflop_vgg(H: int, W: int, images: int = 2) -> float:
+    """2 x multiply-adds of the thirteen convolutions for `images` images of HxW (1503 per 1920x1280 image)."""
+    total, h, w = 0, H, W
+    for group in VGG_GROUPS:
+        total += sum(2 * h * w * cout * cin * 9 for cin, cout in group)
+        h, w = h // 2, w // 2
+    return images * total / 1e9
 
 
 def gflop(H: int, W: int, images: int = 2) -> float:
@@ -65,6 +84,7 @@ def time_calls(f, calls):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--net", choices=("alex", "vgg"), default="alex")
     ap.add_argument("--sizes", default="960x640,1920x1280")
     ap.add_argument("--calls", type=int, default=50)
     ap.add_argument("--rounds", type=int, default=5)
@@ -76,10 +96,15 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_lpips needs a CUDA device")
 
-    import lpips_ref
     from bench_eval import power_limit_w
-    from oracle import lpips_oracle as lo
-    from s3gaussian_b200.lpips import LPIPS
+    if a.net == "vgg":
+        import lpips_vgg_ref as lpips_ref
+        from oracle import lpips_vgg_oracle as lo
+        from s3gaussian_b200.lpips_vgg import LPIPSVGG as LPIPS
+    else:
+        import lpips_ref
+        from oracle import lpips_oracle as lo
+        from s3gaussian_b200.lpips import LPIPS
 
     dev = torch.device("cuda:0")
     feat, lin = lo.random_state_dicts(0)
@@ -113,7 +138,7 @@ def main():
                 calls = a.calls if k != "oracle_fp64" else max(3, a.calls // 10)
                 ms[k].append(time_calls(lambda: f(x, y), calls))
         torch.backends.cudnn.allow_tf32 = default_tf32
-        gf = gflop(H, W)
+        gf = (gflop_vgg if a.net == "vgg" else gflop)(H, W)
         res = {}
         for k, f in arms.items():
             t = float(np.median(ms[k]))
@@ -125,10 +150,10 @@ def main():
         sizes.append({"resolution": f"{W}x{H}", "fp64_value": exact, "arms": res})
 
     render = None
-    if not a.skip_render:
+    if not a.skip_render and a.net == "alex":
         render = bench_render_pixels(a, dev, ours, cudnn(True) if ref is not None else None)
         torch.backends.cudnn.allow_tf32 = default_tf32
-    print(json.dumps({"metric": "LPIPS alex v0.1 ms per call (one image pair)", "gpu": torch.cuda.get_device_name(dev),
+    print(json.dumps({"metric": f"LPIPS {a.net} v0.1 ms per call (one image pair)", "gpu": torch.cuda.get_device_name(dev),
                       "power_limit_w": power_limit_w(), "calls_per_round": a.calls, "rounds": a.rounds,
                       "sizes": sizes, "render_pixels": render}))
 
