@@ -16,7 +16,6 @@
 #include "binning.cuh"
 #include "common.cuh"
 #include "composite.cuh"
-#include "composite_det.cuh"
 #include "preprocess.cuh"
 #define S3G_SCAN_IMPL
 #include "radix_sort.cuh"
@@ -484,8 +483,25 @@ int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f
     return R;
 }
 
-// det: the deterministic backward composite (composite_det.cuh) with det_ws as its workspace, instead of the REDs of
-// render_backward_kernel; everything else, validation included, is shared.
+// one backward composite walk (the default walk takes the RenderBwdArgs part of ra); > 48 KB of dynamic shared memory
+// needs the opt-in, once per (kernel, device)
+template <bool AUX, bool DET>
+int launch_render_backward(const RenderBwdDetArgs& ra, const TileGrid& tg, cudaStream_t stream) {
+    static unsigned long long attr_done = 0;
+    int devid = 0;
+    S3G_CUDA(cudaGetDevice(&devid), "cudaGetDevice");
+    if (devid >= 64 || !((attr_done >> devid) & 1ull)) {
+        S3G_CUDA(cudaFuncSetAttribute(render_backward_kernel<AUX, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)sizeof(RenderBwdSmem<AUX, DET>)),
+                 DET ? "render_backward_det smem attribute" : "render_backward smem attribute");
+        if (devid < 64) attr_done |= 1ull << devid;
+    }
+    render_backward_kernel<AUX, DET><<<dim3(tg.x, tg.y), TILE_PIX, sizeof(RenderBwdSmem<AUX, DET>), stream>>>(ra);
+    return S3G_OK;
+}
+
+// det: the deterministic destination of the backward composite walk (composite.cuh) with det_ws as its workspace,
+// instead of the REDs into grad_rec; everything else, validation included, is shared.
 int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, cudaStream_t stream, bool det,
                   void* det_ws) {
     const int P = s.P, width = s.width, height = s.height, debug = s.debug;
@@ -529,41 +545,24 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
 
     g_timer.begin(1);
     const bool det_walk = det && b.R > 0;
+    RenderBwdDetArgs ra = {};
+    ra.ranges = img.ranges; ra.point_list = bin.point_list; ra.W = width; ra.H = height;
+    ra.bg = s.background; ra.xyAB = geom.xyAB; ra.Cod = geom.Cod; ra.rgb = geom.rgb;
+    ra.final_T = img.final_T; ra.n_contrib = img.n_contrib;
+    ra.dL_dpix = b.dL_dpix; ra.dL_dpix_depth = b.dL_dpix_depth; ra.grad_rec = geom.grad_rec;
+    ra.aux = geom.aux; ra.dL_dpix_aux = b.dL_dpix_aux;
     if (det_walk) {
         // every grad_rec row is written by the gather: no memset
         float4* records = static_cast<float4*>(det_ws);
         uint32_t* base = reinterpret_cast<uint32_t*>(static_cast<char*>(det_ws) + det_records_bytes(b.R));
+        ra.rect = geom.rect; ra.base = base; ra.records = records;
         S3G_MARK(1, "det_base");
         det_base_kernel<<<(P + 255) / 256, 256, 0, stream>>>((uint32_t)P, geom.order_a, geom.offsets, base);
         S3G_STAGE("det_base");
         S3G_MARK(1, "render_backward_det");
-        RenderBwdDetArgs da;
-        RenderBwdArgs& ra = da.b;
-        ra.ranges = img.ranges; ra.point_list = bin.point_list; ra.W = width; ra.H = height;
-        ra.bg = s.background; ra.xyAB = geom.xyAB; ra.Cod = geom.Cod; ra.rgb = geom.rgb;
-        ra.final_T = img.final_T; ra.n_contrib = img.n_contrib;
-        ra.dL_dpix = b.dL_dpix; ra.dL_dpix_depth = b.dL_dpix_depth; ra.grad_rec = nullptr;
-        ra.aux = geom.aux; ra.dL_dpix_aux = b.dL_dpix_aux;
-        da.rect = geom.rect; da.base = base; da.records = records;
-        static unsigned long long attr_done = 0;
-        int devid = 0;
-        S3G_CUDA(cudaGetDevice(&devid), "cudaGetDevice");
-        if (devid >= 64 || !((attr_done >> devid) & 1ull)) {
-            S3G_CUDA(cudaFuncSetAttribute(render_backward_det_kernel<false>,
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)sizeof(RenderBwdDetSmem<false>)),
-                     "render_backward_det smem attribute");
-            S3G_CUDA(cudaFuncSetAttribute(render_backward_det_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)sizeof(RenderBwdDetSmem<true>)),
-                     "render_backward_det smem attribute");
-            if (devid < 64) attr_done |= 1ull << devid;
-        }
-        if (use_aux)
-            render_backward_det_kernel<true>
-                <<<dim3(tg.x, tg.y), TILE_PIX, sizeof(RenderBwdDetSmem<true>), stream>>>(da);
-        else
-            render_backward_det_kernel<false>
-                <<<dim3(tg.x, tg.y), TILE_PIX, sizeof(RenderBwdDetSmem<false>), stream>>>(da);
+        const int rc = use_aux ? launch_render_backward<true, true>(ra, tg, stream)
+                               : launch_render_backward<false, true>(ra, tg, stream);
+        if (rc != S3G_OK) return rc;
         S3G_STAGE("render_backward_det");
         S3G_MARK(1, "grad_rec_gather");
         grad_rec_gather_kernel<<<(unsigned)div_up64((int64_t)P * 4, 256), 256, 0, stream>>>(
@@ -574,32 +573,12 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
         S3G_CUDA(cudaMemsetAsync(geom.grad_rec, 0, (size_t)P * GRAD_REC * sizeof(float), stream),
                  "memset grad_rec");
         S3G_MARK(1, "render_backward");
-    }
-    if (!det_walk && b.R > 0) {
-        RenderBwdArgs ra;
-        ra.ranges = img.ranges; ra.point_list = bin.point_list; ra.W = width; ra.H = height;
-        ra.bg = s.background; ra.xyAB = geom.xyAB; ra.Cod = geom.Cod; ra.rgb = geom.rgb;
-        ra.final_T = img.final_T; ra.n_contrib = img.n_contrib;
-        ra.dL_dpix = b.dL_dpix; ra.dL_dpix_depth = b.dL_dpix_depth; ra.grad_rec = geom.grad_rec;
-        ra.aux = geom.aux; ra.dL_dpix_aux = b.dL_dpix_aux;
-        // > 48 KB of dynamic shared memory needs the opt-in, once per device
-        static unsigned long long attr_done = 0;
-        int devid = 0;
-        S3G_CUDA(cudaGetDevice(&devid), "cudaGetDevice");
-        if (devid >= 64 || !((attr_done >> devid) & 1ull)) {
-            S3G_CUDA(cudaFuncSetAttribute(render_backward_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)sizeof(RenderBwdSmem<false>)),
-                     "render_backward smem attribute");
-            S3G_CUDA(cudaFuncSetAttribute(render_backward_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)sizeof(RenderBwdSmem<true>)),
-                     "render_backward smem attribute");
-            if (devid < 64) attr_done |= 1ull << devid;
+        if (b.R > 0) {
+            const int rc = use_aux ? launch_render_backward<true, false>(ra, tg, stream)
+                                   : launch_render_backward<false, false>(ra, tg, stream);
+            if (rc != S3G_OK) return rc;
+            S3G_STAGE("render_backward");
         }
-        if (use_aux)
-            render_backward_kernel<true><<<dim3(tg.x, tg.y), TILE_PIX, sizeof(RenderBwdSmem<true>), stream>>>(ra);
-        else
-            render_backward_kernel<false><<<dim3(tg.x, tg.y), TILE_PIX, sizeof(RenderBwdSmem<false>), stream>>>(ra);
-        S3G_STAGE("render_backward");
     }
 
     S3G_MARK(1, "preprocess_backward");

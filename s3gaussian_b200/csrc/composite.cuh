@@ -19,9 +19,13 @@
 //    as soon as all warps are;
 //  * backward: two phases per warp - lane = pixel for the sequential recurrences, then
 //    lane = instance for the sums over pixels (moments of X = G dL/dalpha in registers) -
-//    and three vector REDs per (warp, instance) instead of 10 atomics per (pixel,
-//    Gaussian) pair (backward.cu:550-587); see render_backward_kernel.
+//    and one record per (warp, instance) instead of 10 atomics per (pixel, Gaussian) pair
+//    (backward.cu:550-587).  One walk, two destinations for the record: three vector REDs
+//    into grad_rec, or (deterministic backward) per-warp shared-memory partials summed in a
+//    fixed order; see render_backward_kernel.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace s3g {
@@ -430,7 +434,13 @@ struct RenderBwdArgs {
     const float* dL_dpix_depth;  // [1,H,W]
     const float4* aux;           // second colour set (AUX kernels) or NULL
     const float* dL_dpix_aux;    // [3,H,W] or NULL
-    float* grad_rec;             // [P][GRAD_REC], zeroed
+    float* grad_rec;             // [P][GRAD_REC], zeroed (default walk only)
+};
+// the deterministic walk's destination
+struct RenderBwdDetArgs : RenderBwdArgs {
+    const ushort4* rect;         // [P] of the forward
+    const uint32_t* base;        // [P], det_base_kernel
+    float4* records;             // [R][GRAD_REC / 4]
 };
 
 __device__ __forceinline__ float rcp_approx(float x) {
@@ -459,29 +469,88 @@ __device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
 //        dL/dcolour_c = sum w dL/dpix_c        dL/ddepth = sum w dL/dpix_depth
 //  phase 2, lane = (instance slot, half of the rectangle): after BKS survivors the roles flip - every lane walks
 //    16 pixels of ONE instance, accumulating the six pixel-coordinate moments of X (separable: three per pixel,
-//    six per row) and the four w * dL/dpix sums in registers; the halves meet with 10 shuffles, the moments are
-//    shifted to the Gaussian's centre and land as three vector REDs per instance.
+//    six per row) and the four w * dL/dpix sums in registers; the halves meet with 10 shuffles and the moments are
+//    shifted to the Gaussian's centre (bwd_flush).
 //
 // Per surviving (warp, instance) that is ~12 issue slots of reduction instead of the 46-instruction shuffle
 // butterfly + selects of a per-instance warp reduction.
-constexpr int BCB = 128;          // instances per staged batch (backward)
+//
+// The same walk has two destinations for a flushed record (bwd_store):
+//  * default (s3g_rasterize_backward): three vector REDs per (warp, instance) into the Gaussian's grad_rec row, in
+//    whatever order warps and tiles get there - so two calls on the same inputs differ in the last bits;
+//  * deterministic (s3g_rasterize_backward_deterministic, DET): every sum is taken in an order fixed by the inputs.
+//    A flush stores into the warp's shared-memory partial of the batch slot; at the end of each batch of DCB
+//    instances the block adds the eight warps' partials in warp order and writes one record per (tile, instance)
+//    to the workspace at its emit position.  Partials a warp never writes (no surviving pixel, a warp past its last
+//    contributor) stay zero, and instances behind the tile's deepest contributor get a zero record, so no stale
+//    workspace content is ever read.  Around the walk:
+//      - det_base_kernel: base[g] = position of Gaussian g's first tile instance in emit order (the forward's
+//        exclusive scan `offsets`, indexed through the depth order).  Instance (g, tile t) has emit position
+//        base[g] + (row-major index of t in g's rect), exactly as emit_instances_kernel numbered it.
+//      - grad_rec_gather_kernel: every Gaussian's records summed over its tiles in row-major order, written as its
+//        full grad_rec row (this replaces the memset of the default path).
+//    No global atomics anywhere; preprocess_backward then reads grad_rec as it does after the default path.
+constexpr int BCB = 128;          // instances per staged batch (default)
+constexpr int DCB = 64;           // instances per staged batch (deterministic)
 constexpr int BKS = 16;           // survivor slots per warp
 constexpr int BXW_STRIDE = 33;    // float2 row stride of the slot table: conflict-free for both phases
 
-template <bool AUX>
-struct RenderBwdSmem {
-    Rec rec[2][BCB];                       // 12 KB
-    float4 aux[AUX ? 2 : 1][AUX ? BCB : 1];
+// deterministic workspace: [R][GRAD_REC] floats of per-(tile, instance) records in emit order, then [P] uint32 base
+// offsets
+__host__ __device__ inline size_t det_records_bytes(int64_t R) { return (size_t)R * GRAD_REC * sizeof(float); }
+
+__global__ void det_base_kernel(uint32_t P, const uint32_t* __restrict__ order, const uint32_t* __restrict__ offsets,
+                                uint32_t* __restrict__ base) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < P) base[order[k]] = offsets[k];
+}
+
+// emit position of instance (Gaussian g, tile tx, ty): emit_instances_kernel numbers a Gaussian's tiles row-major
+// over its rect, starting at base[g]
+__device__ __forceinline__ size_t det_emit_pos(const ushort4* __restrict__ rect, const uint32_t* __restrict__ base,
+                                               uint32_t g, uint32_t tx, uint32_t ty) {
+    const ushort4 r = rect[g];
+    return (size_t)base[g] + (ty - r.y) * (uint32_t)(r.z - r.x) + (tx - r.x);
+}
+
+// shared memory of the walk, batches of NB instances
+template <bool AUX, int NB>
+struct BwdWalkSmem {
+    Rec rec[2][NB];
+    float4 aux[AUX ? 2 : 1][AUX ? NB : 1];
     float4 dpix_aux[AUX ? 8 : 1][AUX ? 32 : 1];   // dL/dpix of the second image
     float2 xw[8][BKS][BXW_STRIDE];         // 33 KB  {X, w} per (slot, pixel)
     float4 slot_a[8][BKS];                 // {pix.x, pix.y, conic.x, conic.y}
-    float4 slot_b[8][BKS];                 // {conic.z, opacity, -, id bits}
+    float4 slot_b[8][BKS];                 // {conic.z, opacity, batch slot (bits) if DET, id bits}
     float4 dpix[8][32];                    // dL/dpix {r, g, b, depth} of the warp's pixels
+};
+template <bool AUX, bool DET>
+struct RenderBwdSmem : BwdWalkSmem<AUX, BCB> {
+    uint32_t max_contrib;
+};
+template <bool AUX>
+struct RenderBwdSmem<AUX, true> : BwdWalkSmem<AUX, DCB> {
+    float4 part[AUX ? 4 : 3][8][DCB];      // [record quarter][warp][batch slot]; zero unless written this batch
     uint32_t max_contrib;
 };
 
-template <bool AUX>
-__device__ __forceinline__ void bwd_flush(const RenderBwdSmem<AUX>& sm, int warp, int lane, int ns, float cx, float cy,
+// quarter q of a flushed record to its destination: row g of grad_rec, or this warp's partial of batch slot `slot`
+// (DET).  Each batch slot is flushed at most once per warp and batch.
+template <bool AUX, bool DET>
+__device__ __forceinline__ void bwd_store(RenderBwdSmem<AUX, DET>& sm, int warp, float* g, int slot, int q, float4 v) {
+    if constexpr (DET) {
+        sm.part[q][warp][slot] = v;
+    } else {
+        if (q == 3) atomicAdd(g + 4 * q, v.x);
+        else if (q == 2 && !AUX) red_add_v2(g + 4 * q, v.x, v.y);
+        else red_add_v4(g + 4 * q, v.x, v.y, v.z, v.w);
+    }
+}
+
+// lane (j, h) sums slot j's moments over half h of the rectangle; after the shuffles it holds the record's quarters
+// 0 and 2 (h == 0) or 1 and 3 (h == 1, quarter 3 with AUX only) and stores them
+template <bool AUX, bool DET>
+__device__ __forceinline__ void bwd_flush(RenderBwdSmem<AUX, DET>& sm, int warp, int lane, int ns, float cx, float cy,
                                           float ddelx_dx, float ddely_dy, float* __restrict__ grad_rec) {
     const int j = lane & (BKS - 1), h = lane >> 4;
     const float2* row = &sm.xw[warp][j][h * 16];
@@ -536,23 +605,28 @@ __device__ __forceinline__ void bwd_flush(const RenderBwdSmem<AUX>& sm, int warp
         const float syy = fmaf(ey, ey * m00 - 2.f * m01, m02);
         const float sxy = fmaf(ex, ey * m00 - m01, m11 - ey * m10);
         const float o = gb.y, hf = -0.5f * o;
+        // the record's destination: the Gaussian's grad_rec row, or (DET) its batch slot
         float* g = grad_rec + (size_t)__float_as_uint(gb.w) * GRAD_REC;
+        const int slot = __float_as_int(gb.z);
         if (h == 0) {
-            red_add_v4(g, o * ddelx_dx * (-ga.z * sx - ga.w * sy), o * ddely_dy * (-gb.x * sy - ga.w * sx), hf * sxx,
-                       hf * sxy);
-            if (AUX) red_add_v4(g + 8, c2, cd, x0, x1);
-            else red_add_v2(g + 8, c2, cd);
+            bwd_store(sm, warp, g, slot, 0, make_float4(o * ddelx_dx * (-ga.z * sx - ga.w * sy),
+                                                        o * ddely_dy * (-gb.x * sy - ga.w * sx), hf * sxx, hf * sxy));
+            bwd_store(sm, warp, g, slot, 2, make_float4(c2, cd, x0, x1));   // x0 = x1 = 0 without AUX
         } else {
-            red_add_v4(g + 4, hf * syy, m00, c0, c1);
-            if (AUX) atomicAdd(g + 12, x2);
+            bwd_store(sm, warp, g, slot, 1, make_float4(hf * syy, m00, c0, c1));
+            if constexpr (AUX) bwd_store(sm, warp, g, slot, 3, make_float4(x2, 0.f, 0.f, 0.f));
         }
     }
 }
 
-template <bool AUX>
-__global__ void __launch_bounds__(TILE_PIX) render_backward_kernel(RenderBwdArgs a) {
+template <bool AUX, bool DET>
+__global__ void __launch_bounds__(TILE_PIX)
+    render_backward_kernel(std::conditional_t<DET, RenderBwdDetArgs, RenderBwdArgs> args) {
     extern __shared__ __align__(16) unsigned char s_raw[];
-    RenderBwdSmem<AUX>& sm = *reinterpret_cast<RenderBwdSmem<AUX>*>(s_raw);
+    RenderBwdSmem<AUX, DET>& sm = *reinterpret_cast<RenderBwdSmem<AUX, DET>*>(s_raw);
+    const RenderBwdArgs& a = args;
+    constexpr int NB = DET ? DCB : BCB;   // instances per staged batch
+    constexpr int NQ = AUX ? 4 : 3;       // record quarters written
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t tile = blockIdx.y * gridDim.x + blockIdx.x;
@@ -568,6 +642,7 @@ __global__ void __launch_bounds__(TILE_PIX) render_backward_kernel(RenderBwdArgs
     const size_t HW = (size_t)a.H * a.W;
 
     const uint2 range = a.ranges[tile];
+    const int n = (int)(range.y - range.x);
 
     const float T_final = inside ? a.final_T[pix_id] : 0.f;
     float T = T_final;
@@ -594,12 +669,24 @@ __global__ void __launch_bounds__(TILE_PIX) render_backward_kernel(RenderBwdArgs
 
     // only instances below the block's deepest contributor matter (backward.cu:513)
     if (tid == 0) sm.max_contrib = 0;
+    if constexpr (DET)
+        for (int i = tid; i < NQ * 8 * DCB; i += TILE_PIX) (&sm.part[0][0][0])[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     __syncthreads();
     const int warp_max = (int)__reduce_max_sync(0xffffffffu, (uint32_t)last_contributor);
     if (lane == 0 && warp_max > 0) atomicMax(&sm.max_contrib, (uint32_t)warp_max);
     __syncthreads();
     const int m = (int)sm.max_contrib;   // instances [0, m) are walked back to front
-    const int nb = (m + BCB - 1) / BCB;
+    if constexpr (DET) {
+        // instances behind the deepest contributor get a zero record
+        for (int i = m + tid; i < n; i += TILE_PIX) {
+            const uint32_t g = a.point_list[range.x + i];
+            float4* dst =
+                args.records + det_emit_pos(args.rect, args.base, g, blockIdx.x, blockIdx.y) * (GRAD_REC / 4);
+#pragma unroll
+            for (int q = 0; q < NQ; ++q) dst[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+    }
+    const int nb = (m + NB - 1) / NB;
     if (nb == 0) return;
 
     // per-pixel recurrences of backward.cu:529-563.  The reference keeps accum_rec per channel and forms
@@ -610,11 +697,11 @@ __global__ void __launch_bounds__(TILE_PIX) render_backward_kernel(RenderBwdArgs
     const float ddelx_dx = 0.5f * a.W, ddely_dy = 0.5f * a.H;
     int ns = 0;   // filled survivor slots (warp-uniform)
 
-    // slot t of batch b holds list index m-1-(b*BCB+t); threads >= BCB only composite
+    // slot t of batch b holds list index m-1-(b*NB+t); threads >= NB only composite
     uint32_t id_next = 0;
     {
         const int i0 = m - 1 - tid;
-        if (tid < BCB && i0 >= 0) {
+        if (tid < NB && i0 >= 0) {
             const uint32_t id = a.point_list[range.x + i0];
             cp_async16(&sm.rec[0][tid].a, &a.xyAB[id]);
             cp_async16(&sm.rec[0][tid].b, &a.Cod[id]);
@@ -622,28 +709,28 @@ __global__ void __launch_bounds__(TILE_PIX) render_backward_kernel(RenderBwdArgs
             if (AUX) cp_async16(&sm.aux[0][tid], &a.aux[id]);
         }
         cp_async_commit();
-        const int i1 = m - 1 - (BCB + tid);
-        if (tid < BCB && i1 >= 0) id_next = a.point_list[range.x + i1];
+        const int i1 = m - 1 - (NB + tid);
+        if (tid < NB && i1 >= 0) id_next = a.point_list[range.x + i1];
         cp_async_wait_all();
         __syncthreads();
     }
 
     for (int b = 0; b < nb; ++b) {
         const int buf = b & 1;
-        if (tid < BCB) {
-            const int i1 = m - 1 - ((b + 1) * BCB + tid);
+        if (tid < NB) {
+            const int i1 = m - 1 - ((b + 1) * NB + tid);
             if (i1 >= 0) {
                 cp_async16(&sm.rec[buf ^ 1][tid].a, &a.xyAB[id_next]);
                 cp_async16(&sm.rec[buf ^ 1][tid].b, &a.Cod[id_next]);
                 cp_async16(&sm.rec[buf ^ 1][tid].c, &a.rgb[id_next]);
                 if (AUX) cp_async16(&sm.aux[buf ^ 1][tid], &a.aux[id_next]);
             }
-            const int i2 = m - 1 - ((b + 2) * BCB + tid);
+            const int i2 = m - 1 - ((b + 2) * NB + tid);
             if (i2 >= 0) id_next = a.point_list[range.x + i2];
         }
         cp_async_commit();
-        const int top = m - 1 - b * BCB;           // list index of slot 0
-        const int cnt = min(BCB, top + 1);
+        const int top = m - 1 - b * NB;            // list index of slot 0
+        const int cnt = min(NB, top + 1);
         const Rec* rec = sm.rec[buf];
         // the warp has nothing to do for instances at or above warp_max
         if (top - (cnt - 1) < warp_max) {
@@ -696,7 +783,7 @@ __global__ void __launch_bounds__(TILE_PIX) render_backward_kernel(RenderBwdArgs
                     sm.xw[warp][ns][lane] = make_float2(X, w);
                     if (lane == 0) {
                         sm.slot_a[warp][ns] = g0;
-                        sm.slot_b[warp][ns] = g1;
+                        sm.slot_b[warp][ns] = DET ? make_float4(g1.x, g1.y, __int_as_float(jj), g1.w) : g1;
                     }
                     if (++ns == BKS) {
                         __syncwarp();
@@ -706,14 +793,61 @@ __global__ void __launch_bounds__(TILE_PIX) render_backward_kernel(RenderBwdArgs
                     }
                 }
             }
+            // slots never span a deterministic batch: its partials are complete at the barrier below
+            if constexpr (DET) {
+                if (ns) {
+                    __syncwarp();
+                    bwd_flush(sm, warp, lane, ns, cx, cy, ddelx_dx, ddely_dy, a.grad_rec);
+                    __syncwarp();
+                    ns = 0;
+                }
+            }
         }
         cp_async_wait_all();
         __syncthreads();
+        if constexpr (DET) {
+            // quarter q of slot t: the eight warps' partials added in warp order, then zeroed for the next batch
+            const int q = tid / DCB, t = tid % DCB;
+            if (q < NQ && t < cnt) {
+                float4 s = sm.part[q][0][t];
+                sm.part[q][0][t] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+                for (int w = 1; w < 8; ++w) {
+                    const float4 v = sm.part[q][w][t];
+                    sm.part[q][w][t] = make_float4(0.f, 0.f, 0.f, 0.f);
+                    s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+                }
+                const uint32_t g = __float_as_uint(rec[t].b.w);
+                args.records[det_emit_pos(args.rect, args.base, g, blockIdx.x, blockIdx.y) * (GRAD_REC / 4) + q] = s;
+            }
+            __syncthreads();
+        }
     }
-    if (ns) {
+    if (!DET && ns) {
         __syncwarp();
         bwd_flush(sm, warp, lane, ns, cx, cy, ddelx_dx, ddely_dy, a.grad_rec);
     }
+}
+
+// four threads per Gaussian, one record quarter each: the sum over the Gaussian's tiles in row-major order of its
+// rect, written as quarter q of its grad_rec row (quarters >= nq and Gaussians without tiles are written as zeros)
+__global__ void grad_rec_gather_kernel(uint32_t P, int nq, const uint32_t* __restrict__ tiles_touched,
+                                       const uint32_t* __restrict__ base, const float4* __restrict__ records,
+                                       float4* __restrict__ grad_rec) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t g = (uint32_t)(i >> 2);
+    const int q = (int)(i & 3);
+    if (g >= P) return;
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+    const uint32_t nt = tiles_touched[g];
+    if (q < nq && nt) {
+        const float4* r = records + (size_t)base[g] * (GRAD_REC / 4) + q;
+        for (uint32_t k = 0; k < nt; ++k) {
+            const float4 v = r[(size_t)k * (GRAD_REC / 4)];
+            s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+        }
+    }
+    grad_rec[(size_t)g * (GRAD_REC / 4) + q] = s;
 }
 
 }  // namespace s3g
