@@ -66,3 +66,51 @@ def test_deform_oracle_backward(path):
             assert rel(v.grad.numpy(), z[key]) < 1e-4, (k, rel(v.grad.numpy(), z[key]))
             checked += 1
     assert checked >= 20
+
+
+@pytest.mark.parametrize("chunk", [64, 100])
+def test_chunked_oracle_equals_single_pass(chunk):
+    """do.chunked_front (the float64 oracle run in chunks, what the GPU tests use at 500 k and 2 M Gaussians) against one
+    pass over all Gaussians: outputs, input gradients and the plane / Linear gradients that accumulate over the chunks'
+    backward calls.  Chunk sizes that do not divide P, every head on, an SH degree below 3 and an unused output."""
+    reso, multires = (6, 5, 4, 3), (1, 2)
+    st = syn.make_deform_state(4, reso, multires, aabb=((9.0, 4.0, 3.0), (-2.0, -4.0, -3.0)), weight_scale=0.2)
+    flags = dict(no_ds=False, no_dr=False, no_do=False)
+    P = 301
+    g = torch.Generator().manual_seed(9)
+    xyz = torch.tensor([-2.0, -4.0, -3.0]) + torch.tensor([11.0, 8.0, 6.0]) * (torch.rand(P, 3, generator=g) * 1.2 - 0.1)
+    inputs = [v.double() for v in (xyz, torch.randn(P, 3, generator=g) * 0.3 - 2, torch.randn(P, 4, generator=g),
+                                   torch.randn(P, 1, generator=g), torch.randn(P, 16, 3, generator=g) * 0.3)]
+    shapes = ((P, 3), (P, 3), (P, 4), (P, 1), (P, 3), (P, 3), (P, 16, 3), (P, 3))
+    upstream = [torch.randn(*s, generator=g, dtype=torch.float64) for s in shapes]
+    upstream[7] = None
+    campos = torch.tensor([0.3, -0.2, 6.0], dtype=torch.float64)
+
+    def run(c):
+        state = {k: v.double().requires_grad_(k != "deformation_net.grid.aabb") for k, v in st.items()}
+        outs, grads, margins = do.chunked_front(state, inputs, 0.37, campos, 2, upstream, chunk=c, **flags)
+        return outs, grads, {k: v.grad for k, v in state.items() if v.grad is not None}, margins
+
+    ref, mine = run(P), run(chunk)
+    for a, b in zip(ref[0] + ref[1], mine[0] + mine[1]):
+        assert a.shape == b.shape and rel(b.numpy(), a.numpy()) < 1e-12
+    assert set(ref[2]) == set(mine[2]) and len(ref[2]) >= 6 * len(multires) + 20
+    for k in ref[2]:
+        assert rel(mine[2][k].numpy(), ref[2][k].numpy()) < 1e-12, k
+    for k in ref[3]:
+        assert torch.equal(ref[3][k], mine[3][k]), k
+    # the single pass is the plain composition deform_forward -> render_front
+    d = do.deform_forward({k: v.double() for k, v in st.items()}, *inputs, torch.full((P, 1), 0.37, dtype=torch.float64),
+                          **flags)
+    assert torch.equal(ref[0][4], do.render_front(inputs[0], d, campos, 2)["colors_precomp"])
+
+
+def test_chunked_oracle_empty():
+    st = syn.make_deform_state(4, (6, 5, 4, 3), (1,), aabb=((9.0, 4.0, 3.0), (-2.0, -4.0, -3.0)))
+    state = {k: v.double().requires_grad_(k != "deformation_net.grid.aabb") for k, v in st.items()}
+    inputs = [torch.zeros(0, *s, dtype=torch.float64) for s in ((3,), (3,), (4,), (1,), (16, 3))]
+    upstream = [torch.zeros(0, *s, dtype=torch.float64) for s in ((3,), (3,), (4,), (1,), (3,), (3,), (16, 3), (3,))]
+    outs, grads, _ = do.chunked_front(state, inputs, 0.5, torch.zeros(3, dtype=torch.float64), 3, upstream, chunk=7)
+    assert [tuple(o.shape) for o in outs] == [(0, 3), (0, 3), (0, 4), (0, 1), (0, 3), (0, 3), (0, 16, 3), (0, 3)]
+    assert [tuple(x.shape) for x in grads] == [(0, 3), (0, 3), (0, 4), (0, 1), (0, 16, 3)]
+    assert all(v.grad is None or not v.grad.any() for v in state.values())
