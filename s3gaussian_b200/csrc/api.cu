@@ -442,7 +442,7 @@ int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f
         S3G_STAGE("tile sort");
 
         S3G_MARK(0, "render_forward");
-        RenderFwdArgs ra;
+        RenderSplitArgs ra = {};
         ra.ranges = img.ranges; ra.point_list = bin.point_list; ra.W = width; ra.H = height;
         ra.xyAB = geom.xyAB; ra.Cod = geom.Cod; ra.rgb = geom.rgb; ra.bg = s.background;
         ra.final_T = img.final_T; ra.n_contrib = img.n_contrib;
@@ -451,19 +451,18 @@ int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f
         // flow colour sets are gathered from the caller's [P,4] arrays directly (no copy into geom.aux)
         AuxSet a1 = {reinterpret_cast<const float4*>(f.flow_colors[1]), f.out_flow[1]};
         if (f.n_flow > 0) { ra.aux = reinterpret_cast<const float4*>(f.flow_colors[0]); ra.out_aux = f.out_flow[0]; }
+        ra.out_color_d = f.out_color_d; ra.out_depth_d = f.out_depth_d;
+        ra.out_color_s = f.out_color_s; ra.out_depth_s = f.out_depth_s;
+        ra.group_count = geom.scan_misc + 4; ra.P = (uint32_t)P;
+        const int na = f.n_flow == 2 ? 2 : (f.colors_aux || f.n_flow == 1) ? 1 : 0;   // extra colour sets
         const dim3 grid(tg.x, tg.y);
-        if (split) {
-            RenderSplitArgs sa;
-            sa.f = ra;
-            sa.out_color_d = f.out_color_d; sa.out_depth_d = f.out_depth_d;
-            sa.out_color_s = f.out_color_s; sa.out_depth_s = f.out_depth_s;
-            sa.group_count = geom.scan_misc + 4; sa.P = (uint32_t)P;
-            if (f.n_flow == 2) render_forward_split_kernel<2><<<grid, TILE_PIX, 0, stream>>>(sa, a1);
-            else if (f.n_flow == 1) render_forward_split_kernel<1><<<grid, TILE_PIX, 0, stream>>>(sa, a1);
-            else render_forward_split_kernel<0><<<grid, TILE_PIX, 0, stream>>>(sa, a1);
-        } else if (f.colors_aux || f.n_flow == 1) render_forward_kernel<1><<<grid, TILE_PIX, 0, stream>>>(ra, a1);
-        else if (f.n_flow == 2) render_forward_kernel<2><<<grid, TILE_PIX, 0, stream>>>(ra, a1);
-        else render_forward_kernel<0><<<grid, TILE_PIX, 0, stream>>>(ra, a1);
+        if (split) {   // the plain walks take the RenderFwdArgs part of ra
+            if (na == 2) render_forward_kernel<2, true><<<grid, TILE_PIX, 0, stream>>>(ra, a1);
+            else if (na == 1) render_forward_kernel<1, true><<<grid, TILE_PIX, 0, stream>>>(ra, a1);
+            else render_forward_kernel<0, true><<<grid, TILE_PIX, 0, stream>>>(ra, a1);
+        } else if (na == 2) render_forward_kernel<2, false><<<grid, TILE_PIX, 0, stream>>>(ra, a1);
+        else if (na == 1) render_forward_kernel<1, false><<<grid, TILE_PIX, 0, stream>>>(ra, a1);
+        else render_forward_kernel<0, false><<<grid, TILE_PIX, 0, stream>>>(ra, a1);
         S3G_STAGE("render_forward");
         S3G_MARK(0, nullptr);
 

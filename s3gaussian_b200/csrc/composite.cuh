@@ -17,6 +17,8 @@
 //    (forward.cu:328-366) is what makes it issue-bound;
 //  * a warp leaves the loop as soon as all its pixels are saturated, the block
 //    as soon as all warps are;
+//  * forward: one walk for the training image, the extra colour sets (feature or
+//    flow images) and the static/dynamic decomposition; see render_forward_kernel;
 //  * backward: two phases per warp - lane = pixel for the sequential recurrences, then
 //    lane = instance for the sums over pixels (moments of X = G dL/dalpha in registers) -
 //    and one record per (warp, instance) instead of 10 atomics per (pixel, Gaussian) pair
@@ -76,7 +78,7 @@ struct RenderFwdArgs {
 };
 
 // The second extra colour set of a two-set walk (the two flow images of an evaluation walk).  It is a kernel parameter
-// of its own so that RenderFwdArgs and RenderSplitArgs keep their layout, and the kernels with fewer sets their code.
+// of its own so that the forward's argument structs keep their layout, and the kernels with fewer sets their code.
 struct AuxSet {
     const float4* colors;    // [P], rgb in .xyz, indexed by Gaussian
     float* out;              // [3,H,W]
@@ -99,14 +101,36 @@ struct __align__(16) Rec {
     float4 c;   // r, g, b, depth
 };
 
-// NA extra colour sets are composited in the same walk, each with the colour image's weights and background: the
-// feature image of render(render_feat=True) (train.py:373; NA = 1) or the flow images of an evaluation walk (NA = 1
-// or 2) - the reference runs its whole rasterizer again on identical geometry for each of them.
-template <int NA>
-__global__ void __launch_bounds__(TILE_PIX) render_forward_kernel(RenderFwdArgs a, AuxSet a1) {
+// the split walk's outputs: the dynamic and static subset images
+struct RenderSplitArgs : RenderFwdArgs {
+    float* out_color_d;              // [3,H,W] dynamic subset
+    float* out_depth_d;
+    float* out_color_s;              // [3,H,W] static subset
+    float* out_depth_s;
+    const uint32_t* group_count;     // dynamic Gaussians (device); a pass over no Gaussians leaves a zero image
+    uint32_t P;
+};
+
+// {dynamic Gaussians, P} of a split walk; the epilogue reads them before its stores, which may alias group_count
+__device__ __forceinline__ uint2 split_counts(const RenderFwdArgs&) { return make_uint2(0u, 0u); }
+__device__ __forceinline__ uint2 split_counts(const RenderSplitArgs& s) { return make_uint2(*s.group_count, s.P); }
+
+// One walk over a tile's sorted list composites the colour image and depth (with final_T and n_contrib), and also:
+//  * NA extra colour sets with the colour image's weights and background: the feature image of render(render_feat=True)
+//    (train.py:373; NA = 1) or the flow images of an evaluation walk (NA = 1 or 2), for each of which the reference
+//    runs its whole rasterizer again on identical geometry;
+//  * SPLIT: the dynamic and static subset images of render(return_decomposition=True).  A subset pass would produce
+//    the same preprocess records and, the depth and tile sorts being stable, the full tile lists without the other
+//    group's entries - so every instance blends into the full set and into its own group's set (bit 31 of Cod.w, set
+//    by the preprocess), each set running the same per-pixel sequence on its own T and alive flag.  Each image is what
+//    a separate pass over its subset computes; the walk ends when all three sets are saturated.
+template <int NA, bool SPLIT>
+__global__ void __launch_bounds__(TILE_PIX)
+    render_forward_kernel(std::conditional_t<SPLIT, RenderSplitArgs, RenderFwdArgs> args, AuxSet a1) {
     static_assert(NA >= 0 && NA <= 2, "at most two extra colour sets");
     __shared__ Rec s_rec[2][CB];
     __shared__ float4 s_aux[NA ? NA : 1][NA ? 2 : 1][NA ? CB : 1];
+    const RenderFwdArgs& a = args;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t tile = blockIdx.y * gridDim.x + blockIdx.x;
@@ -124,11 +148,14 @@ __global__ void __launch_bounds__(TILE_PIX) render_forward_kernel(RenderFwdArgs 
     const int n = (int)(range.y - range.x);
     const int nb = (n + CB - 1) / CB;
 
-    float T = 1.0f;
+    // full image, and (SPLIT) dynamic (_d) and static (_s) accumulators
+    float T = 1.0f, Td = 1.0f, Ts = 1.0f;
     uint32_t last_contributor = 0;
     float C0 = 0.f, C1 = 0.f, C2 = 0.f, D = 0.f;
+    float C0d = 0.f, C1d = 0.f, C2d = 0.f, Dd = 0.f;
+    float C0s = 0.f, C1s = 0.f, C2s = 0.f, Ds = 0.f;
     float A[NA ? NA : 1][3] = {};
-    bool alive = inside;
+    bool alive = inside, alive_d = inside, alive_s = inside;
 
     // prologue: gather batch 0, fetch the id of batch 1
     uint32_t id_next = 0;
@@ -160,7 +187,7 @@ __global__ void __launch_bounds__(TILE_PIX) render_forward_kernel(RenderFwdArgs 
 
         const int cnt = min(CB, n - b * CB);
         const Rec* rec = s_rec[buf];
-        bool warp_done = !__any_sync(0xffffffffu, alive);
+        bool warp_done = !__any_sync(0xffffffffu, SPLIT ? alive || alive_d || alive_s : alive);
         if (!warp_done) {
             for (int c0 = 0; c0 < cnt; c0 += 32) {
                 const int j = c0 + lane;
@@ -183,12 +210,15 @@ __global__ void __launch_bounds__(TILE_PIX) render_forward_kernel(RenderFwdArgs 
                     const float4 g0 = r.a;
                     const float4 g1 = r.b;
                     const float4 col = r.c;
+                    const bool dyn = (__float_as_uint(g1.w) >> 31) != 0;   // SPLIT: the instance's group
                     const float dx = g0.x - pixx, dy = g0.y - pixy;
                     const float power = -0.5f * (g0.z * dx * dx + g1.x * dy * dy) - g0.w * dx * dy;
                     const float alpha = min(0.99f, g1.y * expf(power));
-                    const float test_T = T * (1 - alpha);
                     // forward.cu:339-354: skip power > 0, skip alpha < 1/255, stop at T < 1e-4
-                    const bool ok = alive && !(power > 0.0f) && !(alpha < 1.0f / 255.0f);
+                    const bool vis = !(power > 0.0f) && !(alpha < 1.0f / 255.0f);
+                    const float test_T = T * (1 - alpha);
+                    // alive && vis (spelled out for the plain walk: through vis, nvcc 12.9 reorders its predicates)
+                    const bool ok = SPLIT ? alive && vis : alive && !(power > 0.0f) && !(alpha < 1.0f / 255.0f);
                     const bool stop = ok && (test_T < 0.0001f);
                     const bool blend = ok && !stop;
                     // weight alpha * T once (the reference multiplies feature * alpha * T per channel,
@@ -208,163 +238,9 @@ __global__ void __launch_bounds__(TILE_PIX) render_forward_kernel(RenderFwdArgs 
                     T = blend ? test_T : T;
                     last_contributor = blend ? idx_base + (uint32_t)bit : last_contributor;
                     alive = alive && !stop;
-                }
-                if (!__any_sync(0xffffffffu, alive)) {
-                    warp_done = true;
-                    break;
-                }
-            }
-        }
-        cp_async_wait_all();
-        if (__syncthreads_and(warp_done)) break;
-    }
-
-    if (inside) {
-        const size_t HW = (size_t)a.H * a.W;
-        a.final_T[pix_id] = T;
-        a.n_contrib[pix_id] = last_contributor;
-        a.out_color[0 * HW + pix_id] = C0 + T * a.bg[0];
-        a.out_color[1 * HW + pix_id] = C1 + T * a.bg[1];
-        a.out_color[2 * HW + pix_id] = C2 + T * a.bg[2];
-        a.out_depth[pix_id] = D;
-#pragma unroll
-        for (int k = 0; k < NA; ++k) {
-            float* o = aux_out(a, a1, k);
-            o[0 * HW + pix_id] = A[k][0] + T * a.bg[0];
-            o[1 * HW + pix_id] = A[k][1] + T * a.bg[1];
-            o[2 * HW + pix_id] = A[k][2] + T * a.bg[2];
-        }
-    }
-}
-
-// ---- static / dynamic decomposition (forward only) ----------------------------------------------------------------
-// render(return_decomposition=True) composites the full image, the dynamic subset and the static subset.  A subset
-// pass would produce the same preprocess records and, the depth and tile sorts being stable, the full tile lists with
-// the other group's entries removed - so one walk over the full lists with three accumulator sets gives all three
-// images.  Every instance blends into the full set and into its own group's set (bit 31 of Cod.w, set by the
-// preprocess); each set runs the per-pixel sequence of render_forward_kernel on its own T and alive flag, so each image
-// is what a separate pass over that subset computes.  The walk ends when all three sets are saturated.  NA extra colour
-// sets (the flow images of an evaluation walk) blend into the full image's accumulators as in render_forward_kernel.
-struct RenderSplitArgs {
-    RenderFwdArgs f;                 // full image (+ final_T / n_contrib, as the plain forward)
-    float* out_color_d;              // [3,H,W] dynamic subset
-    float* out_depth_d;
-    float* out_color_s;              // [3,H,W] static subset
-    float* out_depth_s;
-    const uint32_t* group_count;     // dynamic Gaussians (device); a pass over no Gaussians leaves a zero image
-    uint32_t P;
-};
-
-template <int NA>
-__global__ void __launch_bounds__(TILE_PIX) render_forward_split_kernel(RenderSplitArgs sa, AuxSet a1) {
-    static_assert(NA >= 0 && NA <= 2, "at most two extra colour sets");
-    __shared__ Rec s_rec[2][CB];
-    __shared__ float4 s_aux[NA ? NA : 1][NA ? 2 : 1][NA ? CB : 1];
-    const RenderFwdArgs& a = sa.f;
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t tile = blockIdx.y * gridDim.x + blockIdx.x;
-    const int X0 = blockIdx.x * TILE_X + (warp & 1) * SUB_W;
-    const int Y0 = blockIdx.y * TILE_Y + (warp >> 1) * SUB_H;
-    const int px = X0 + (lane & 7), py = Y0 + (lane >> 3);
-    const bool inside = px < a.W && py < a.H;
-    const float pixx = (float)px, pixy = (float)py;
-    const uint32_t pix_id = (uint32_t)a.W * py + px;
-    const float rx0 = (float)X0, rx1 = (float)(X0 + SUB_W - 1);
-    const float ry0 = (float)Y0, ry1 = (float)(Y0 + SUB_H - 1);
-
-    const uint2 range = a.ranges[tile];
-    const int n = (int)(range.y - range.x);
-    const int nb = (n + CB - 1) / CB;
-
-    // full image, dynamic (_d) and static (_s) accumulators
-    float T = 1.0f, Td = 1.0f, Ts = 1.0f;
-    uint32_t last_contributor = 0;
-    float C0 = 0.f, C1 = 0.f, C2 = 0.f, D = 0.f;
-    float C0d = 0.f, C1d = 0.f, C2d = 0.f, Dd = 0.f;
-    float C0s = 0.f, C1s = 0.f, C2s = 0.f, Ds = 0.f;
-    float A[NA ? NA : 1][3] = {};
-    bool alive = inside, alive_d = inside, alive_s = inside;
-
-    uint32_t id_next = 0;
-    if (tid < n) {
-        const uint32_t id = a.point_list[range.x + tid];
-        cp_async16(&s_rec[0][tid].a, &a.xyAB[id]);
-        cp_async16(&s_rec[0][tid].b, &a.Cod[id]);
-        cp_async16(&s_rec[0][tid].c, &a.rgb[id]);
-#pragma unroll
-        for (int k = 0; k < NA; ++k) cp_async16(&s_aux[k][0][tid], &aux_colors(a, a1, k)[id]);
-    }
-    cp_async_commit();
-    if (CB + tid < n) id_next = a.point_list[range.x + CB + tid];
-    cp_async_wait_all();
-    __syncthreads();
-
-    for (int b = 0; b < nb; ++b) {
-        const int buf = b & 1;
-        if ((b + 1) * CB + tid < n) {
-            cp_async16(&s_rec[buf ^ 1][tid].a, &a.xyAB[id_next]);
-            cp_async16(&s_rec[buf ^ 1][tid].b, &a.Cod[id_next]);
-            cp_async16(&s_rec[buf ^ 1][tid].c, &a.rgb[id_next]);
-#pragma unroll
-            for (int k = 0; k < NA; ++k) cp_async16(&s_aux[k][buf ^ 1][tid], &aux_colors(a, a1, k)[id_next]);
-        }
-        cp_async_commit();
-        if ((b + 2) * CB + tid < n) id_next = a.point_list[range.x + (b + 2) * CB + tid];
-
-        const int cnt = min(CB, n - b * CB);
-        const Rec* rec = s_rec[buf];
-        bool warp_done = !__any_sync(0xffffffffu, alive || alive_d || alive_s);
-        if (!warp_done) {
-            for (int c0 = 0; c0 < cnt; c0 += 32) {
-                const int j = c0 + lane;
-                bool pass = false;
-                if (j < cnt) {
-                    const float4 g0 = rec[j].a;
-                    const float4 g1 = rec[j].b;
-                    const float q = rect_min_q(g0.z, g0.w, g1.x, g0.x - rx1, g0.x - rx0,
-                                               g0.y - ry1, g0.y - ry0);
-                    pass = !(q > g1.z);
-                }
-                uint32_t mask = __ballot_sync(0xffffffffu, pass);
-                const uint32_t idx_base = (uint32_t)(b * CB + c0 + 1);
-                while (mask) {
-                    const int bit = __ffs(mask) - 1;
-                    mask &= mask - 1;
-                    const Rec& r = rec[c0 + bit];
-                    const float4 g0 = r.a;
-                    const float4 g1 = r.b;
-                    const float4 col = r.c;
-                    const bool dyn = (__float_as_uint(g1.w) >> 31) != 0;
-                    const float dx = g0.x - pixx, dy = g0.y - pixy;
-                    const float power = -0.5f * (g0.z * dx * dx + g1.x * dy * dy) - g0.w * dx * dy;
-                    const float alpha = min(0.99f, g1.y * expf(power));
-                    const bool vis = !(power > 0.0f) && !(alpha < 1.0f / 255.0f);
-                    // full image: the sequence of render_forward_kernel
-                    {
-                        const float test_T = T * (1 - alpha);
-                        const bool ok = alive && vis;
-                        const bool stop = ok && (test_T < 0.0001f);
-                        const bool blend = ok && !stop;
-                        const float wgt = blend ? alpha * T : 0.0f;
-                        C0 = fmaf(col.x, wgt, C0);
-                        C1 = fmaf(col.y, wgt, C1);
-                        C2 = fmaf(col.z, wgt, C2);
-                        D = fmaf(col.w, wgt, D);
-#pragma unroll
-                        for (int k = 0; k < NA; ++k) {
-                            const float4 ax = s_aux[k][buf][c0 + bit];
-                            A[k][0] = fmaf(ax.x, wgt, A[k][0]);
-                            A[k][1] = fmaf(ax.y, wgt, A[k][1]);
-                            A[k][2] = fmaf(ax.z, wgt, A[k][2]);
-                        }
-                        T = blend ? test_T : T;
-                        last_contributor = blend ? idx_base + (uint32_t)bit : last_contributor;
-                        alive = alive && !stop;
-                    }
-                    // the instance's own group: the same sequence on that group's accumulators (selected, never
-                    // multiplied by zero, so the other group's image sees nothing of this instance)
-                    {
+                    if constexpr (SPLIT) {
+                        // the instance's own group: the same sequence on that group's accumulators (selected, never
+                        // multiplied by zero, so the other group's image sees nothing of this instance)
                         const float Tg = dyn ? Td : Ts;
                         const bool alive_g = dyn ? alive_d : alive_s;
                         const float test_T = Tg * (1 - alpha);
@@ -382,7 +258,7 @@ __global__ void __launch_bounds__(TILE_PIX) render_forward_split_kernel(RenderSp
                         else     { C0s = n0; C1s = n1; C2s = n2; Ds = nd; Ts = nT; alive_s = nalive; }
                     }
                 }
-                if (!__any_sync(0xffffffffu, alive || alive_d || alive_s)) {
+                if (!__any_sync(0xffffffffu, SPLIT ? alive || alive_d || alive_s : alive)) {
                     warp_done = true;
                     break;
                 }
@@ -394,22 +270,24 @@ __global__ void __launch_bounds__(TILE_PIX) render_forward_split_kernel(RenderSp
 
     if (inside) {
         const size_t HW = (size_t)a.H * a.W;
-        const uint32_t nd = *sa.group_count;
-        const bool any_d = nd > 0, any_s = nd < sa.P;
+        const uint2 gc = split_counts(args);
+        const bool any_d = gc.x > 0, any_s = gc.x < gc.y;   // a pass over no Gaussians leaves a zero image
         a.final_T[pix_id] = T;
         a.n_contrib[pix_id] = last_contributor;
         a.out_color[0 * HW + pix_id] = C0 + T * a.bg[0];
         a.out_color[1 * HW + pix_id] = C1 + T * a.bg[1];
         a.out_color[2 * HW + pix_id] = C2 + T * a.bg[2];
         a.out_depth[pix_id] = D;
-        sa.out_color_d[0 * HW + pix_id] = any_d ? C0d + Td * a.bg[0] : 0.f;
-        sa.out_color_d[1 * HW + pix_id] = any_d ? C1d + Td * a.bg[1] : 0.f;
-        sa.out_color_d[2 * HW + pix_id] = any_d ? C2d + Td * a.bg[2] : 0.f;
-        sa.out_depth_d[pix_id] = Dd;
-        sa.out_color_s[0 * HW + pix_id] = any_s ? C0s + Ts * a.bg[0] : 0.f;
-        sa.out_color_s[1 * HW + pix_id] = any_s ? C1s + Ts * a.bg[1] : 0.f;
-        sa.out_color_s[2 * HW + pix_id] = any_s ? C2s + Ts * a.bg[2] : 0.f;
-        sa.out_depth_s[pix_id] = Ds;
+        if constexpr (SPLIT) {
+            args.out_color_d[0 * HW + pix_id] = any_d ? C0d + Td * a.bg[0] : 0.f;
+            args.out_color_d[1 * HW + pix_id] = any_d ? C1d + Td * a.bg[1] : 0.f;
+            args.out_color_d[2 * HW + pix_id] = any_d ? C2d + Td * a.bg[2] : 0.f;
+            args.out_depth_d[pix_id] = Dd;
+            args.out_color_s[0 * HW + pix_id] = any_s ? C0s + Ts * a.bg[0] : 0.f;
+            args.out_color_s[1 * HW + pix_id] = any_s ? C1s + Ts * a.bg[1] : 0.f;
+            args.out_color_s[2 * HW + pix_id] = any_s ? C2s + Ts * a.bg[2] : 0.f;
+            args.out_depth_s[pix_id] = Ds;
+        }
 #pragma unroll
         for (int k = 0; k < NA; ++k) {
             float* o = aux_out(a, a1, k);
