@@ -8,24 +8,24 @@ namespace {
 // prepared-weight table of the wgmma decoder
 void build_tc_table(const DNet& d, TcTable& t, TcPrepArgs* prep) {
     int off = 0;
-    auto put = [&](int id, const float* W, int N, int K, int ld = 0) {
+    auto put = [&](int id, const float* W, int N, int K, int ld) {
         if (!W || K <= 0) { t.off[id] = -1; t.npad[id] = 0; t.k[id] = 0; if (prep) { prep->W[id] = nullptr; prep->n[id] = 0; prep->ld[id] = 0; } return; }
         const int np = (N + 15) & ~15;
         t.off[id] = off; t.npad[id] = np; t.k[id] = K;
         off += 2 * np * K;
-        if (prep) { prep->W[id] = W; prep->n[id] = N; prep->ld[id] = ld ? ld : K; }
+        if (prep) { prep->W[id] = W; prep->n[id] = N; prep->ld[id] = ld; }
     };
-    {   // the feature layer as two K-halves (deform_tc.cuh: TL_FEAT / TL_FEATB)
-        const int KF = FD * d.L, KA = KF < 64 ? KF : 64;
-        put(TL_FEAT, d.w_feat, 64, KA, KF);
-        put(TL_FEATB, d.w_feat ? d.w_feat + KA : nullptr, 64, KF - KA, KF);
+    for (int id = 0; id < TL_LAYERS; ++id) {
+        const float* W = layer_on(d, id) ? layer_w(d, id) : nullptr;
+        const int N = kLayers[id].n, K = layer_k(id, d.L);
+        if (id == TL_FEAT) {    // the feature layer as two K-halves (deform_tc.cuh: TL_FEAT / TL_FEATB)
+            const int KA = K < 64 ? K : 64;
+            put(TL_FEAT, W, N, KA, K);
+            put(TL_FEATB, W + KA, N, K - KA, K);
+        } else {
+            put(id, W, N, K, K);
+        }
     }
-    put(TL_POS1, d.pos.w1, 64, 64); put(TL_POS2, d.pos.w1 ? d.pos.w2 : nullptr, 3, 64);
-    put(TL_SCL1, d.scl.w1, 64, 64); put(TL_SCL2, d.scl.w1 ? d.scl.w2 : nullptr, 3, 64);
-    put(TL_ROT1, d.rot.w1, 64, 64); put(TL_ROT2, d.rot.w1 ? d.rot.w2 : nullptr, 4, 64);
-    put(TL_OPA1, d.opa.w1, 64, 64); put(TL_OPA2, d.opa.w1 ? d.opa.w2 : nullptr, 1, 64);
-    put(TL_SHS1, d.shs.w1, 64, 64); put(TL_SHS2, d.shs.w1 ? d.shs.w2 : nullptr, 48, 64);
-    put(TL_D0, d.w_d0, 64, 64); put(TL_D2, d.w_d0 ? d.w_d2 : nullptr, 64, 64); put(TL_D4, d.w_d0 ? d.w_d4 : nullptr, 3, 64);
     t.total = off;
 }
 int deform_grid(int ntiles, int ctas_per_sm = 1) {
@@ -76,11 +76,7 @@ int s3g_deform_forward_save(const s3g_deform_net* net, int P, const float* xyz, 
         t.o_dx = dx; t.o_dshs = dshs; t.o_feat = feat; t.features = features;
         t.acts = acts;
         t.act_stride = (size_t)((P + 127) / 128) * 128 * 64;
-        {
-            int slot[AK_COUNT];
-            act_slots(a.net, slot);
-            for (int i = 0; i < AK_COUNT; ++i) t.act_slot[i] = slot[i];
-        }
+        act_slots(a.net, t.act_slot);
         TcPrepArgs pp;
         build_tc_table(a.net, t.tab, &pp);
         pp.tab = t.tab;

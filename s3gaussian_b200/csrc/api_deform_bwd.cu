@@ -9,14 +9,11 @@ namespace {
 int make_offsets(const DNet& d, GradOff& o) {
     int t = 0;
     auto take = [&](int n) { int r = t; t += (n + 3) & ~3; return r; };
-    auto head = [&](const Head2& h, int k, int (&dst)[4]) {
-        if (h.w1) { dst[0] = take(64 * 64); dst[1] = take(64); dst[2] = take(k * 64); dst[3] = take(k); }
-        else { dst[0] = dst[1] = dst[2] = dst[3] = -1; }
-    };
-    o.w_feat = take(64 * FD * d.L); o.b_feat = take(64);
-    head(d.pos, 3, o.pos); head(d.scl, 3, o.scl); head(d.rot, 4, o.rot); head(d.opa, 1, o.opa); head(d.shs, 48, o.shs);
-    if (d.w_d0) { o.d0w = take(4096); o.d0b = take(64); o.d2w = take(4096); o.d2b = take(64); o.d4w = take(192); o.d4b = take(3); }
-    else { o.d0w = o.d0b = o.d2w = o.d2b = o.d4w = o.d4b = -1; }
+    for (int id = 0; id < TL_LAYERS; ++id) {
+        const bool on = layer_on(d, id);
+        grad_off(o, kLayers[id].ow) = on ? take(kLayers[id].n * layer_k(id, d.L)) : -1;
+        grad_off(o, kLayers[id].ob) = on ? take(kLayers[id].n) : -1;
+    }
     o.total = t;
     return t;
 }
@@ -42,7 +39,7 @@ extern "C" {
 size_t s3g_deform_saved_bytes(const s3g_deform_net* net, int P) {
     DNet d;
     if (to_dnet(net, d) != S3G_OK || P <= 0) return 0;
-    int slot[AK_COUNT];
+    int slot[ACT_KINDS];
     return (size_t)act_slots(d, slot) * ((size_t)((P + 127) / 128) * 128 * 64) * sizeof(float);
 }
 
@@ -108,18 +105,11 @@ int s3g_deform_backward_saved(const s3g_deform_net* net, int P, const float* xyz
         r.seg[r.nseg++] = ReduceSeg{dst, off, count};
         return true;
     };
-    bool ok = seg(grads->w_feat, a.off.w_feat, 64 * FD * d.L) && seg(grads->b_feat, a.off.b_feat, 64);
-    auto hseg = [&](const int (&o)[4], float* w1, float* b1, float* w2, float* b2, int k) {
-        return seg(w1, o[0], 4096) && seg(b1, o[1], 64) && seg(w2, o[2], k * 64) && seg(b2, o[3], k);
-    };
-    ok = ok && hseg(a.off.pos, grads->w_pos1, grads->b_pos1, grads->w_pos2, grads->b_pos2, 3);
-    ok = ok && hseg(a.off.scl, grads->w_scl1, grads->b_scl1, grads->w_scl2, grads->b_scl2, 3);
-    ok = ok && hseg(a.off.rot, grads->w_rot1, grads->b_rot1, grads->w_rot2, grads->b_rot2, 4);
-    ok = ok && hseg(a.off.opa, grads->w_opa1, grads->b_opa1, grads->w_opa2, grads->b_opa2, 1);
-    ok = ok && hseg(a.off.shs, grads->w_shs1, grads->b_shs1, grads->w_shs2, grads->b_shs2, 48);
-    ok = ok && seg(grads->w_dino0, a.off.d0w, 4096) && seg(grads->b_dino0, a.off.d0b, 64) &&
-         seg(grads->w_dino2, a.off.d2w, 4096) && seg(grads->b_dino2, a.off.d2b, 64) &&
-         seg(grads->w_dino4, a.off.d4w, 192) && seg(grads->b_dino4, a.off.d4b, 3);
+    bool ok = true;
+    for (int id = 0; id < TL_LAYERS && ok; ++id) {
+        const DeformLayer& l = kLayers[id];
+        ok = seg(grads->*l.gw, grad_off(a.off, l.ow), l.n * layer_k(id, d.L)) && seg(grads->*l.gb, grad_off(a.off, l.ob), l.n);
+    }
     if (!ok) return fail(S3G_ERR_ARG, "deform_backward: null Linear gradient for an enabled layer");
     if (P > 0) {
         const size_t smem = DeformBwdSmem::floats(d.L) * sizeof(float);

@@ -43,6 +43,10 @@ struct DNet {                     // device-side view of s3g_deform_net
     Head2 pos, scl, rot, opa, shs;
     const float *w_d0, *b_d0, *w_d2, *b_d2, *w_d4, *b_d4;
 };
+// ids of the Linear layers (deform_host.cuh: DeformLayer describes each), plus TL_FEATB: the second K-half of the
+// feature layer in the wgmma forward's weight table (deform_tc.cuh: TcTable)
+enum { TL_FEAT = 0, TL_POS1, TL_POS2, TL_SCL1, TL_SCL2, TL_ROT1, TL_ROT2, TL_OPA1, TL_OPA2, TL_SHS1, TL_SHS2,
+       TL_D0, TL_D2, TL_D4, TL_FEATB, TL_COUNT };
 
 // plane k samples coordinates (a,b): (0,1),(0,2),(0,3),(1,2),(1,3),(2,3) - compile-time so that
 // unrolled loops index register arrays statically
@@ -550,7 +554,7 @@ struct DeformBwdArgs {
     float* partial;      // [gridDim.x][off.total]
     const float* features;   // [P][32L] from the forward
     const float* acts;       // hidden activations kept by the wgmma forward (layout: DeformTcArgs::acts)
-    int act_slot[8];         // deform_host.cuh: AK_H, AK_POS, AK_SCL, AK_ROT, AK_OPA, AK_SHS, AK_D0, AK_D2; -1 = absent
+    int act_slot[8];         // slot of h, pos, scl, rot, opa, shs, d0, d2 (deform_host.cuh: act_slots), -1 = absent
     size_t act_stride;       // floats per slot = ceil(P / 128) * 128 * 64
     float* dfeatures;        // [P][32L] dL/d(features), consumed by hexplane_scatter_kernel
     GradOff off;
@@ -615,6 +619,28 @@ __device__ __forceinline__ void feat_layers_bwd(const DeformBwdSmem& sm, const D
     dw_accum<64, KF, false>(sm.DH, HS, sm.F, FS, part + off.w_feat, part + off.b_feat);
     __syncthreads();
     tile_linear_T<KF, 64, TL_ASSIGN>(sm.DH, HS, pipe, sm.A, FS, nullptr, 0);
+}
+
+// One of the scales, rotation and opacity heads (k = 3, 4, 1 outputs) in deform_backward_kernel.  When the head is on,
+// fetch() starts the next kept activation, and the head's outputs are recomputed into G[11..11+k) from its kept hidden
+// layer Ab; act_bwd(on) writes the activation backward to Dout and to the d_* output; then, when the head is on, its
+// two layers' gradients go into the partial buffer (GradOff row o) and the delta is pushed back into DH.
+template <class Fetch, class ActBwd>
+__device__ __forceinline__ void small_head_bwd(int k, const Head2& h, const int (&o)[4], float* Ab, Fetch fetch,
+                                               ActBwd act_bwd, const DeformBwdSmem& sm, float* part, WPipe& pipe) {
+    const bool on = h.w1 != nullptr;
+    if (on) {
+        fetch();
+        tile_small_out(Ab, HS, h.w2, h.b2, k, sm.G, 16, 11);
+        __syncthreads();
+    }
+    act_bwd(on);
+    __syncthreads();
+    if (on) {
+        small_head_backward(sm.Dout, k, Ab, HS, h.w2, part + o[2], part + o[3], sm.D1, HS);
+        dw_accum<64, 64, true>(sm.D1, HS, sm.H, HS, part + o[0], part + o[1]);
+        tile_linear_T<64, 64, TL_ACCUM_MASK>(sm.D1, HS, pipe, sm.DH, HS, sm.H, HS);
+    }
 }
 
 // The hidden activations (h and every head's hidden layer) are read from the buffer the wgmma forward filled, so a
@@ -699,15 +725,7 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
             dw_accum<64, 64, true>(sm.D1, HS, sm.H, HS, part + a.off.pos[0], part + a.off.pos[1]);
             tile_linear_T<64, 64, TL_ACCUM_MASK>(sm.D1, HS, pipe, sm.DH, HS, sm.H, HS);
         }
-        // ---- scales head: scales_act = exp(scales + ds) ---------------------------
-        {
-            const bool on = n.scl.w1 != nullptr;
-            float* Ab = abuf[2];
-            if (on) {
-                fetch_after(2, g0);
-                tile_small_out(Ab, HS, n.scl.w2, n.scl.b2, 3, sm.G, 16, 11);     // ds -> G[11..13]
-                __syncthreads();
-            }
+        small_head_bwd(3, n.scl, a.off.scl, abuf[2], [&] { fetch_after(2, g0); }, [&](bool on) {      // scales_act = exp(scales + ds)
             if (tid < DT * 4) {
                 const int g = tid >> 2, c = tid & 3, gi = g0 + g;
                 float d = 0.f;
@@ -718,22 +736,8 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
                 }
                 sm.Dout[tid] = d;
             }
-            __syncthreads();
-            if (on) {
-                small_head_backward(sm.Dout, 3, Ab, HS, n.scl.w2, part + a.off.scl[2], part + a.off.scl[3], sm.D1, HS);
-                dw_accum<64, 64, true>(sm.D1, HS, sm.H, HS, part + a.off.scl[0], part + a.off.scl[1]);
-                tile_linear_T<64, 64, TL_ACCUM_MASK>(sm.D1, HS, pipe, sm.DH, HS, sm.H, HS);
-            }
-        }
-        // ---- rotation head: rot_act = normalize(rot + dr) --------------------------
-        {
-            const bool on = n.rot.w1 != nullptr;
-            float* Ab = abuf[3];
-            if (on) {
-                fetch_after(3, g0);
-                tile_small_out(Ab, HS, n.rot.w2, n.rot.b2, 4, sm.G, 16, 11);     // dr -> G[11..14]
-                __syncthreads();
-            }
+        }, sm, part, pipe);
+        small_head_bwd(4, n.rot, a.off.rot, abuf[3], [&] { fetch_after(3, g0); }, [&](bool on) {      // rot_act = normalize(rot + dr)
             if (tid < DT) {
                 const int g = tid, gi = g0 + g;
                 float dq[4] = {0.f, 0.f, 0.f, 0.f};
@@ -762,22 +766,8 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
 #pragma unroll
                 for (int i = 0; i < 4; ++i) sm.Dout[g * 4 + i] = dq[i];
             }
-            __syncthreads();
-            if (on) {
-                small_head_backward(sm.Dout, 4, Ab, HS, n.rot.w2, part + a.off.rot[2], part + a.off.rot[3], sm.D1, HS);
-                dw_accum<64, 64, true>(sm.D1, HS, sm.H, HS, part + a.off.rot[0], part + a.off.rot[1]);
-                tile_linear_T<64, 64, TL_ACCUM_MASK>(sm.D1, HS, pipe, sm.DH, HS, sm.H, HS);
-            }
-        }
-        // ---- opacity head: opacity_act = sigmoid(opacity + do) ---------------------
-        {
-            const bool on = n.opa.w1 != nullptr;
-            float* Ab = abuf[4];
-            if (on) {
-                fetch_after(4, g0);
-                tile_small_out(Ab, HS, n.opa.w2, n.opa.b2, 1, sm.G, 16, 11);     // do -> G[11]
-                __syncthreads();
-            }
+        }, sm, part, pipe);
+        small_head_bwd(1, n.opa, a.off.opa, abuf[4], [&] { fetch_after(4, g0); }, [&](bool on) {      // opacity_act = sigmoid(opacity + do)
             if (tid < DT * 4) {
                 const int g = tid >> 2, c = tid & 3, gi = g0 + g;
                 float d = 0.f;
@@ -789,13 +779,7 @@ __global__ void __launch_bounds__(DTHREADS, 1) deform_backward_kernel(const __gr
                 }
                 sm.Dout[tid] = d;
             }
-            __syncthreads();
-            if (on) {
-                small_head_backward(sm.Dout, 1, Ab, HS, n.opa.w2, part + a.off.opa[2], part + a.off.opa[3], sm.D1, HS);
-                dw_accum<64, 64, true>(sm.D1, HS, sm.H, HS, part + a.off.opa[0], part + a.off.opa[1]);
-                tile_linear_T<64, 64, TL_ACCUM_MASK>(sm.D1, HS, pipe, sm.DH, HS, sm.H, HS);
-            }
-        }
+        }, sm, part, pipe);
         // ---- shs head + SH->RGB backward ---------------------------------------------
         {
             const bool on = n.shs.w1 != nullptr;

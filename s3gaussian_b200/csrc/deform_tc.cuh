@@ -1,6 +1,6 @@
 // deform_tc.cuh - the deformation decoder (forward) on the Hopper warpgroup tensor cores (wgmma).
 //
-// Same arithmetic as the decoder stage of deform.cuh (3xTF32: hi*hi + hi*lo + lo*hi, fp32
+// Same 3xTF32 arithmetic as the backward decoder of deform.cuh (hi*hi + hi*lo + lo*hi, fp32
 // accumulate) but the dense layers are wgmma.mma_async instructions reading both operands from
 // shared memory instead of warp-level mma.sync:
 //
@@ -25,11 +25,9 @@ namespace s3g {
 
 constexpr int TCM = 128;          // Gaussians per tile = two wgmma M = 64 halves
 
-// layer ids in the prepared-weight table
+// prepared-weight table, indexed by the layer ids TL_* (deform.cuh)
 // (TL_FEAT / TL_FEATB: the feature layer is run as two K-halves, columns [0,64) and [64,32L) of its weight, so that no
 //  operand tile is wider than 64 columns: 96 KB of shared memory per CTA instead of 192 KB, two CTAs per SM)
-enum { TL_FEAT = 0, TL_POS1, TL_POS2, TL_SCL1, TL_SCL2, TL_ROT1, TL_ROT2, TL_OPA1, TL_OPA2, TL_SHS1, TL_SHS2,
-       TL_D0, TL_D2, TL_D4, TL_FEATB, TL_COUNT };
 struct TcTable {
     int off[TL_COUNT];     // float offset of the layer's [hi | lo] block in the prepared buffer, -1 = absent
     int npad[TL_COUNT];    // rows padded to a multiple of 16
@@ -76,7 +74,7 @@ struct DeformTcArgs {
     // (cp.async.bulk shared -> global) issued next to that layer's MMAs - no per-thread stores.  The hi operand
     // holds the fp32 value itself (the tensor core ignores the low mantissa bits), so the copy is exact.
     float* acts;
-    int act_slot[8];           // slot of H, pos, scl, rot, opa, shs, d0, d2 (deform_host.cuh: AK_*), -1 = absent
+    int act_slot[8];           // slot of H, pos, scl, rot, opa, shs, d0, d2 (deform_host.cuh: act_slots), -1 = absent
     size_t act_stride;         // floats per slot = ceil(P / 128) * 128 * 64
 };
 

@@ -31,41 +31,36 @@ from . import _lib
 MAX_LEVELS = 8
 _PF = C.POINTER(C.c_float)
 
-_LINEAR_FIELDS = [
-    ("w_feat", "b_feat"),
-    ("w_pos1", "b_pos1"), ("w_pos2", "b_pos2"),
-    ("w_scl1", "b_scl1"), ("w_scl2", "b_scl2"),
-    ("w_rot1", "b_rot1"), ("w_rot2", "b_rot2"),
-    ("w_opa1", "b_opa1"), ("w_opa2", "b_opa2"),
-    ("w_shs1", "b_shs1"), ("w_shs2", "b_shs2"),
-    ("w_dino0", "b_dino0"), ("w_dino2", "b_dino2"), ("w_dino4", "b_dino4"),
+# every Linear the kernels read: reference module path, s3g_deform_net field suffix (w_<suffix>, b_<suffix>) and the
+# args switch of its head (None: always on; a no_* switch turns the head off, feat_head turns it on)
+_LAYERS = [
+    ("feature_out.0", "feat", None),
+    ("pos_deform.1", "pos1", "no_dx"), ("pos_deform.3", "pos2", "no_dx"),
+    ("scales_deform.1", "scl1", "no_ds"), ("scales_deform.3", "scl2", "no_ds"),
+    ("rotations_deform.1", "rot1", "no_dr"), ("rotations_deform.3", "rot2", "no_dr"),
+    ("opacity_deform.1", "opa1", "no_do"), ("opacity_deform.3", "opa2", "no_do"),
+    ("shs_deform.1", "shs1", "no_dshs"), ("shs_deform.3", "shs2", "no_dshs"),
+    ("dino_head.0", "dino0", "feat_head"), ("dino_head.2", "dino2", "feat_head"), ("dino_head.4", "dino4", "feat_head"),
 ]
-_FLAT = [f for pair in _LINEAR_FIELDS for f in pair]
+_FIELDS = [(f"{wb}_{suffix}", C.c_void_p) for _, suffix, _ in _LAYERS for wb in ("w", "b")]
+
+
+def _head_on(args, switch):
+    if switch is None:
+        return True
+    if switch.startswith("no_"):
+        return not getattr(args, switch)
+    return getattr(args, switch, True)
 
 
 class CNet(C.Structure):           # s3g_deform_net (include/s3g_b200.h)
-    _fields_ = ([("num_levels", C.c_int), ("feat_dim", C.c_int), ("width", C.c_int),
-                 ("reso", (C.c_int * 4) * MAX_LEVELS), ("planes", (C.c_void_p * 6) * MAX_LEVELS),
-                 ("aabb", C.c_float * 6)] + [(f, C.c_void_p) for f in _FLAT])
+    _fields_ = [("num_levels", C.c_int), ("feat_dim", C.c_int), ("width", C.c_int),
+                ("reso", (C.c_int * 4) * MAX_LEVELS), ("planes", (C.c_void_p * 6) * MAX_LEVELS),
+                ("aabb", C.c_float * 6)] + _FIELDS
 
 
 class CNetGrads(C.Structure):      # s3g_deform_net_grads
-    _fields_ = [("planes", (C.c_void_p * 6) * MAX_LEVELS)] + [(f, C.c_void_p) for f in _FLAT]
-
-
-# reference module path of every Linear the kernels read -> C struct field prefix
-_LAYERS = {
-    "feature_out.0": ("w_feat", "b_feat"),
-    "pos_deform.1": ("w_pos1", "b_pos1"), "pos_deform.3": ("w_pos2", "b_pos2"),
-    "scales_deform.1": ("w_scl1", "b_scl1"), "scales_deform.3": ("w_scl2", "b_scl2"),
-    "rotations_deform.1": ("w_rot1", "b_rot1"), "rotations_deform.3": ("w_rot2", "b_rot2"),
-    "opacity_deform.1": ("w_opa1", "b_opa1"), "opacity_deform.3": ("w_opa2", "b_opa2"),
-    "shs_deform.1": ("w_shs1", "b_shs1"), "shs_deform.3": ("w_shs2", "b_shs2"),
-    "dino_head.0": ("w_dino0", "b_dino0"), "dino_head.2": ("w_dino2", "b_dino2"),
-    "dino_head.4": ("w_dino4", "b_dino4"),
-}
-_HEAD_FLAG = {"pos_deform": "no_dx", "scales_deform": "no_ds", "rotations_deform": "no_dr",
-              "opacity_deform": "no_do", "shs_deform": "no_dshs"}
+    _fields_ = [("planes", (C.c_void_p * 6) * MAX_LEVELS)] + _FIELDS
 
 
 def _p(t):
@@ -222,22 +217,14 @@ class deform_network(nn.Module):
                                   opacity, shs, *self._param_list())
 
     # ---- plumbing ------------------------------------------------------------
-    def _enabled(self, layer_name):
-        head = layer_name.split(".")[0]
-        if head in _HEAD_FLAG:
-            return not getattr(self.args, _HEAD_FLAG[head])
-        if head == "dino_head":
-            return getattr(self.args, "feat_head", True)
-        return True
-
     def _named_hot_params(self):
         d = self.deformation_net
         out = []
         for li, gp in enumerate(d.grid.grids):
             for ci, p in enumerate(gp):
                 out.append((f"grid.{li}.{ci}", p))
-        for lname in _LAYERS:
-            if not self._enabled(lname):
+        for lname, _, switch in _LAYERS:
+            if not _head_on(self.args, switch):
                 continue
             mod = d
             for part in lname.split("."):
@@ -266,8 +253,9 @@ class deform_network(nn.Module):
         aabb = d.grid.aabb.detach().reshape(-1).tolist()
         for i in range(6):
             cnet.aabb[i] = aabb[i]
-        for lname, (wf, bf) in _LAYERS.items():
-            on = self._enabled(lname)
+        for lname, suffix, switch in _LAYERS:
+            on = _head_on(self.args, switch)
+            wf, bf = "w_" + suffix, "b_" + suffix
             setattr(cnet, wf, tensors_by_name[lname + ".weight"].data_ptr() if on else None)
             setattr(cnet, bf, tensors_by_name[lname + ".bias"].data_ptr() if on else None)
             if grads is not None:
