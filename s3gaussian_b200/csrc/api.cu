@@ -112,6 +112,23 @@ int tile_key_bits(uint32_t tiles) {
     while (b < 32 && (tiles >> b) != 0) ++b;
     return b < 1 ? 1 : b;
 }
+
+// Launch a per-Gaussian kernel that stages each warp's SH rows (3 * M floats per Gaussian) in dynamic shared memory
+// when use_sh: k16 for rows of 16 coefficients, whose length it knows at compile time, k0 for any other M or no SH.
+template <class Args>
+int launch_sh_rows(void (*k16)(Args), void (*k0)(Args), const Args& args, int grid, int threads, int M, bool use_sh,
+                   const char* what, cudaStream_t stream) {
+    const size_t smem = use_sh ? (size_t)threads * row_stride(3 * M) * sizeof(float) : 0;
+    if (smem > 200 * 1024) return fail(S3G_ERR_ARG, (std::string(what) + ": too many SH coefficients").c_str());
+    if (use_sh && M == 16) {
+        k16<<<grid, threads, smem, stream>>>(args);
+        return S3G_OK;
+    }
+    if (smem > 48 * 1024)
+        S3G_CUDA(cudaFuncSetAttribute(k0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "smem attribute");
+    k0<<<grid, threads, smem, stream>>>(args);
+    return S3G_OK;
+}
 }  // namespace
 namespace s3g {
 int api_fail(int code, const char* what, cudaError_t e) {
@@ -335,19 +352,10 @@ int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f
     S3G_CUDA(cudaMemsetAsync(geom.scan_status, 0, geom.zero_bytes, stream), "memset scan/sort state");
     S3G_MARK(0, "preprocess_forward");
     {
-        const bool use_sh = s.colors_precomp == nullptr;
-        const size_t smem = use_sh ? (size_t)(PRE_THREADS / 32) * 32 * row_stride(3 * s.M) * sizeof(float) : 0;
-        if (smem > 200 * 1024) return fail(S3G_ERR_ARG, "forward: too many SH coefficients");
-        const int grid = (P + PRE_THREADS - 1) / PRE_THREADS;
-        if (use_sh && s.M == 16) {
-            preprocess_forward_kernel<16><<<grid, PRE_THREADS, smem, stream>>>(pa);
-        } else {
-            if (smem > 48 * 1024)
-                S3G_CUDA(cudaFuncSetAttribute(preprocess_forward_kernel<0>,
-                                              cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                         "smem attribute");
-            preprocess_forward_kernel<0><<<grid, PRE_THREADS, smem, stream>>>(pa);
-        }
+        const int rc = launch_sh_rows(preprocess_forward_kernel<16>, preprocess_forward_kernel<0>, pa,
+                                      (P + PRE_THREADS - 1) / PRE_THREADS, PRE_THREADS, s.M,
+                                      s.colors_precomp == nullptr, "forward", stream);
+        if (rc != S3G_OK) return rc;
     }
     S3G_STAGE("preprocess_forward");
     S3G_MARK(0, "depth_sort");
@@ -606,28 +614,12 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
         pb.sink.off_scale = sink->off_scales; pb.sink.off_rot = sink->off_rotations;
     }
     {
-        const size_t smem = use_sh ? (size_t)(PRE_THREADS / 32) * 32 * row_stride(3 * s.M) * sizeof(float) : 0;
-        if (smem > 200 * 1024) return fail(S3G_ERR_ARG, "backward: too many SH coefficients");
         const int grid = (P + PRE_THREADS - 1) / PRE_THREADS;
-        if (sink) {
-            if (use_sh && s.M == 16) {
-                preprocess_backward_kernel<16, true><<<grid, PRE_THREADS, smem, stream>>>(pb);
-            } else {
-                if (smem > 48 * 1024)
-                    S3G_CUDA(cudaFuncSetAttribute(preprocess_backward_kernel<0, true>,
-                                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                             "smem attribute");
-                preprocess_backward_kernel<0, true><<<grid, PRE_THREADS, smem, stream>>>(pb);
-            }
-        } else if (use_sh && s.M == 16) {
-            preprocess_backward_kernel<16><<<grid, PRE_THREADS, smem, stream>>>(pb);
-        } else {
-            if (smem > 48 * 1024)
-                S3G_CUDA(cudaFuncSetAttribute(preprocess_backward_kernel<0>,
-                                              cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                         "smem attribute");
-            preprocess_backward_kernel<0><<<grid, PRE_THREADS, smem, stream>>>(pb);
-        }
+        const int rc = sink ? launch_sh_rows(preprocess_backward_kernel<16, true>, preprocess_backward_kernel<0, true>,
+                                             pb, grid, PRE_THREADS, s.M, use_sh, "backward", stream)
+                            : launch_sh_rows(preprocess_backward_kernel<16>, preprocess_backward_kernel<0>, pb, grid,
+                                             PRE_THREADS, s.M, use_sh, "backward", stream);
+        if (rc != S3G_OK) return rc;
     }
     S3G_STAGE("preprocess_backward");
     S3G_MARK(1, nullptr);
@@ -710,18 +702,12 @@ int s3g_rasterize_camera_backward(const s3g_raster_scene* scene, const s3g_raste
     ca.dL_dmean2D = b.dL_dmean2D; ca.dL_dconic = b.dL_dconic; ca.dL_ddepth = b.dL_ddepth; ca.dL_dcolor = b.dL_dcolor;
     ca.partial = static_cast<double*>(workspace);
     ca.nblocks = camera_grad_blocks(P);
-    const size_t smem = campos ? (size_t)CAM_THREADS * row_stride(3 * s.M) * sizeof(float) : 0;
-    if (smem > 200 * 1024) return fail(S3G_ERR_ARG, "camera_backward: too many SH coefficients");
-    if (!campos) {
-        camera_grad_partial_kernel<0, false><<<ca.nblocks, CAM_THREADS, 0, stream>>>(ca);
-    } else if (s.M == 16) {
-        camera_grad_partial_kernel<16, true><<<ca.nblocks, CAM_THREADS, smem, stream>>>(ca);
+    if (campos) {
+        const int rc = launch_sh_rows(camera_grad_partial_kernel<16, true>, camera_grad_partial_kernel<0, true>, ca,
+                                      ca.nblocks, CAM_THREADS, s.M, true, "camera_backward", stream);
+        if (rc != S3G_OK) return rc;
     } else {
-        if (smem > 48 * 1024)
-            S3G_CUDA(cudaFuncSetAttribute(camera_grad_partial_kernel<0, true>,
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                     "smem attribute");
-        camera_grad_partial_kernel<0, true><<<ca.nblocks, CAM_THREADS, smem, stream>>>(ca);
+        camera_grad_partial_kernel<0, false><<<ca.nblocks, CAM_THREADS, 0, stream>>>(ca);
     }
     S3G_STAGE("camera_grad_partial");
     camera_grad_finish_kernel<<<1, 32 * CAM_NCOMP, 0, stream>>>(ca.partial, ca.nblocks, out->dL_dviewmatrix,

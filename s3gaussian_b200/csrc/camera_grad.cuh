@@ -7,10 +7,10 @@
 //   t     = viewmatrix x~          -> J(t) (with the 1.3 tanfov clamp), depth = t.z
 //   W     = viewmatrix[:3,:3]      -> cov2D = J W Sigma W^T J^T + 0.3 I -> conic
 //   dir   = x - campos             -> SH colour (the clamped mask zeroes a channel)
-// The gradient with respect to t is the one preprocess_backward_kernel forms for dL_dmean3D (the same zero gradient
-// through the clamped components of t), so these gradients and the per-Gaussian ones describe the same function.
-// The SH derivative is restated here rather than shared with preprocess_backward_kernel, whose machine code does not
-// change for this pass.
+// The derivatives up to dL/dt, dL/d(J W) and dL/d(normalised dir) are preprocess_backward_kernel's own: load_cov3d,
+// ewa_jacobian, cov2d_backward and sh_ddir in preprocess.cuh (the same zero gradient through the clamped components
+// of t), so these gradients and the per-Gaussian ones describe the same function.  What is left here is the chain
+// rule from those to the camera's entries.
 //
 // Summation order, fixed by P alone: each warp adds its 32 Gaussians' contributions with one xor butterfly in double
 // and keeps a running sum per component over the block's CAM_ITERS rounds; a block adds its warps in warp order; the
@@ -54,46 +54,6 @@ struct CamBwdArgs {
 
 __host__ __device__ inline int camera_grad_blocks(int P) { return (int)div_up64(P, CAM_GAUSS_PER_BLOCK); }
 
-// dL/d(unnormalised dir) of the SH colour (backward.cu:20-139 restated; the same expressions as the preprocess backward)
-__device__ __forceinline__ float3 camera_sh_ddir(int deg, const float3 dir_orig, const float* sh, uint8_t cl,
-                                                 const float* dL_dcolor) {
-    const float len = sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
-    const float x = dir_orig.x / len, y = dir_orig.y / len, z = dir_orig.z / len;
-    const float dRGB[3] = {(cl & 1) ? 0.f : dL_dcolor[0], (cl & 2) ? 0.f : dL_dcolor[1], (cl & 4) ? 0.f : dL_dcolor[2]};
-    float ddir[3] = {0.f, 0.f, 0.f};
-    if (deg > 0) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-#define SH(i) sh[(i) * 3 + c]
-            float dx_ = -kC1 * SH(3);
-            float dy_ = -kC1 * SH(1);
-            float dz_ = kC1 * SH(2);
-            if (deg > 1) {
-                dx_ += kC2[0] * y * SH(4) + kC2[2] * 2.f * -x * SH(6) + kC2[3] * z * SH(7) + kC2[4] * 2.f * x * SH(8);
-                dy_ += kC2[0] * x * SH(4) + kC2[1] * z * SH(5) + kC2[2] * 2.f * -y * SH(6) + kC2[4] * 2.f * -y * SH(8);
-                dz_ += kC2[1] * y * SH(5) + kC2[2] * 2.f * 2.f * z * SH(6) + kC2[3] * x * SH(7);
-                if (deg > 2) {
-                    const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-                    dx_ += (kC3[0] * SH(9) * 3.f * 2.f * xy + kC3[1] * SH(10) * yz + kC3[2] * SH(11) * -2.f * xy +
-                            kC3[3] * SH(12) * -3.f * 2.f * xz + kC3[4] * SH(13) * (-3.f * xx + 4.f * zz - yy) +
-                            kC3[5] * SH(14) * 2.f * xz + kC3[6] * SH(15) * 3.f * (xx - yy));
-                    dy_ += (kC3[0] * SH(9) * 3.f * (xx - yy) + kC3[1] * SH(10) * xz +
-                            kC3[2] * SH(11) * (-3.f * yy + 4.f * zz - xx) + kC3[3] * SH(12) * -3.f * 2.f * yz +
-                            kC3[4] * SH(13) * -2.f * xy + kC3[5] * SH(14) * -2.f * yz + kC3[6] * SH(15) * -3.f * 2.f * xy);
-                    dz_ += (kC3[1] * SH(10) * xy + kC3[2] * SH(11) * 4.f * 2.f * yz +
-                            kC3[3] * SH(12) * 3.f * (2.f * zz - xx - yy) + kC3[4] * SH(13) * 4.f * 2.f * xz +
-                            kC3[5] * SH(14) * (xx - yy));
-                }
-            }
-#undef SH
-            ddir[0] += dx_ * dRGB[c];
-            ddir[1] += dy_ * dRGB[c];
-            ddir[2] += dz_ * dRGB[c];
-        }
-    }
-    return dnormvdv3(dir_orig, make_float3(ddir[0], ddir[1], ddir[2]));
-}
-
 // One visible Gaussian's contribution to the CAM_NCOMP components.  sh: its staged coefficient row when CAMPOS.
 template <bool CAMPOS>
 __device__ __forceinline__ void camera_contrib(const CamBwdArgs& a, const Cam& cam, int idx, const float* sh,
@@ -102,60 +62,19 @@ __device__ __forceinline__ void camera_contrib(const CamBwdArgs& a, const Cam& c
     const float* proj = cam.proj;
     const float3 mean = {a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2]};
     float cov3D[6];
-    if (a.cov3D_precomp) {
-#pragma unroll
-        for (int i = 0; i < 6; ++i) cov3D[i] = a.cov3D_precomp[6 * idx + i];
-    } else {
-        const float3 s = {a.scales[3 * idx], a.scales[3 * idx + 1], a.scales[3 * idx + 2]};
-        const float4 q = reinterpret_cast<const float4*>(a.rotations)[idx];
-        cov3d_from_scale_rot(s, a.scale_modifier, q, cov3D);
-    }
+    float3 scl;
+    float4 rot;
+    load_cov3d(a, idx, cov3D, scl, rot);
     const float4 dconic = reinterpret_cast<const float4*>(a.dL_dconic)[idx];   // {x, y, 0, z}
 
-    // ---- conic -> cov2D -> T = J W (the preprocess backward's expressions), then J and W ----------------------------
-    float3 t = xform4x3(mean, view);
-    const float limx = 1.3f * a.tan_fovx, limy = 1.3f * a.tan_fovy;
-    const float txtz = t.x / t.z, tytz = t.y / t.z;
-    t.x = min(limx, max(-limx, txtz)) * t.z;
-    t.y = min(limy, max(-limy, tytz)) * t.z;
-    const float x_grad_mul = txtz < -limx || txtz > limx ? 0.f : 1.f;
-    const float y_grad_mul = tytz < -limy || tytz > limy ? 0.f : 1.f;
-    const float h_x = a.focal_x, h_y = a.focal_y;
-    const M3 J = m3(h_x / t.z, 0.0f, -(h_x * t.x) / (t.z * t.z), 0.0f, h_y / t.z, -(h_y * t.y) / (t.z * t.z), 0.f, 0.f,
-                    0.f);
-    const M3 W = m3(view[0], view[4], view[8], view[1], view[5], view[9], view[2], view[6], view[10]);
-    const M3 Vrk = m3(cov3D[0], cov3D[1], cov3D[2], cov3D[1], cov3D[3], cov3D[4], cov3D[2], cov3D[4], cov3D[5]);
-    const M3 T = m3_mul(W, J);
-    const M3 cov2D = m3_mul(m3_mul(m3_t(T), m3_t(Vrk)), T);
-    const float ca = cov2D.c[0][0] + 0.3f, cb = cov2D.c[0][1], cc = cov2D.c[1][1] + 0.3f;
-    const float denom = ca * cc - cb * cb;
-    float dL_da = 0, dL_db = 0, dL_dc = 0;
-    const float denom2inv = 1.0f / ((denom * denom) + 0.0000001f);
-    if (denom2inv != 0) {
-        dL_da = denom2inv * (-cc * cc * dconic.x + 2 * cb * cc * dconic.y + (denom - ca * cc) * dconic.w);
-        dL_dc = denom2inv * (-ca * ca * dconic.w + 2 * ca * cb * dconic.y + (denom - ca * cc) * dconic.x);
-        dL_db = denom2inv * 2 * (cb * cc * dconic.x - (denom + 2 * cb * cb) * dconic.y + ca * cb * dconic.w);
-    }
+    // ---- conic -> cov2D -> T = J W and t, as the preprocess backward ------------------------------------------------
+    const EwaJacobian e = ewa_jacobian(a, mean, view);
+    const Cov2dGrad g = cov2d_backward(a, e, cov3D, make_float3(dconic.x, dconic.y, dconic.w));
+    const M3& J = e.J;
     // dT[k][j] = dL/d(J W)[k][j] (row k of the 2x3 product, column j): T.c[k][j] in the glm layout
-    float dT[2][3];
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-        const float s0 = T.c[0][0] * Vrk.c[j][0] + T.c[0][1] * Vrk.c[j][1] + T.c[0][2] * Vrk.c[j][2];
-        const float s1 = T.c[1][0] * Vrk.c[j][0] + T.c[1][1] * Vrk.c[j][1] + T.c[1][2] * Vrk.c[j][2];
-        dT[0][j] = 2 * s0 * dL_da + s1 * dL_db;
-        dT[1][j] = 2 * s1 * dL_dc + s0 * dL_db;
-    }
-    const float dL_dJ00 = W.c[0][0] * dT[0][0] + W.c[0][1] * dT[0][1] + W.c[0][2] * dT[0][2];
-    const float dL_dJ02 = W.c[2][0] * dT[0][0] + W.c[2][1] * dT[0][1] + W.c[2][2] * dT[0][2];
-    const float dL_dJ11 = W.c[1][0] * dT[1][0] + W.c[1][1] * dT[1][1] + W.c[1][2] * dT[1][2];
-    const float dL_dJ12 = W.c[2][0] * dT[1][0] + W.c[2][1] * dT[1][1] + W.c[2][2] * dT[1][2];
-    const float tz = 1.f / t.z;
-    const float tz2 = tz * tz;
-    const float tz3 = tz2 * tz;
+    const float (&dT)[2][3] = g.dL_dT;
     // dL/dt, the depth term (depth = t.z) included
-    const float dt[3] = {x_grad_mul * -h_x * tz2 * dL_dJ02, y_grad_mul * -h_y * tz2 * dL_dJ12,
-                         -h_x * tz2 * dL_dJ00 - h_y * tz2 * dL_dJ11 + (2 * h_x * t.x) * tz3 * dL_dJ02 +
-                             (2 * h_y * t.y) * tz3 * dL_dJ12 + a.dL_ddepth[idx]};
+    const float dt[3] = {g.dL_dt.x, g.dL_dt.y, g.dL_dt.z + a.dL_ddepth[idx]};
     // viewmatrix entry 4c + r = V[r][c]: t_r = sum_c V[r][c] x~_c, and (J W)[k][c] = sum_r J[k][r] V[r][c] with
     // J[0] = (J.c[0][0], 0, J.c[0][2]), J[1] = (0, J.c[1][1], J.c[1][2])
     const float xt[4] = {mean.x, mean.y, mean.z, 1.f};
@@ -180,7 +99,12 @@ __device__ __forceinline__ void camera_contrib(const CamBwdArgs& a, const Cam& c
     // ---- SH colour through dir = x - campos ---------------------------------------------------------------------------
     if (CAMPOS) {
         const float3 dir_orig = {mean.x - cam.campos[0], mean.y - cam.campos[1], mean.z - cam.campos[2]};
-        const float3 dm = camera_sh_ddir(a.D, dir_orig, sh, a.clamped[idx], a.dL_dcolor + 3 * idx);
+        const float len = sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
+        const uint8_t cl = a.clamped[idx];
+        const float* dcol = a.dL_dcolor + 3 * idx;
+        const float dRGB[3] = {(cl & 1) ? 0.f : dcol[0], (cl & 2) ? 0.f : dcol[1], (cl & 4) ? 0.f : dcol[2]};
+        const float3 dm =
+            dnormvdv3(dir_orig, sh_ddir(a.D, dir_orig.x / len, dir_orig.y / len, dir_orig.z / len, sh, dRGB));
         c[24] = -dm.x;
         c[25] = -dm.y;
         c[26] = -dm.z;

@@ -127,27 +127,120 @@ __device__ __forceinline__ void cov3d_from_scale_rot(const float3 scale, float m
     cov3D[5] = sig(2, 2);
 }
 
-// forward.cu:74-113
-__device__ __forceinline__ float3 cov2d_ewa(const float3& mean, float focal_x, float focal_y,
-                                            float tan_fovx, float tan_fovy, const float* cov3D,
-                                            const float* view) {
+// Gaussian idx's six cov3D values: the precomputed ones, or those of its scale and rotation, which are returned in
+// scl / rot (zeros when precomputed).  a: PreFwdArgs, PreBwdArgs or CamBwdArgs.
+template <class Args>
+__device__ __forceinline__ void load_cov3d(const Args& a, int idx, float cov3D[6], float3& scl, float4& rot) {
+    scl = {0.f, 0.f, 0.f};
+    rot = {0.f, 0.f, 0.f, 0.f};
+    if (a.cov3D_precomp != nullptr) {
+#pragma unroll
+        for (int i = 0; i < 6; ++i) cov3D[i] = a.cov3D_precomp[6 * idx + i];
+    } else {
+        scl = {a.scales[3 * idx], a.scales[3 * idx + 1], a.scales[3 * idx + 2]};
+        rot = reinterpret_cast<const float4*>(a.rotations)[idx];
+        cov3d_from_scale_rot(scl, a.scale_modifier, rot, cov3D);
+    }
+}
+
+// The EWA projection's Jacobian at a mean (forward.cu:78-97): t = the camera-space mean with x/z and y/z clamped to
+// 1.3 tanfov, J = d(image)/dt at that t, W = the view rotation, T = W J.  x/y_grad_mul are 0 where the clamp is
+// active, so the backward passes no gradient through a clamped component.  a: PreFwdArgs, PreBwdArgs or CamBwdArgs.
+struct EwaJacobian {
+    float x_grad_mul, y_grad_mul;
+    float3 t;
+    M3 J, W, T;
+};
+template <class Args>
+__device__ __forceinline__ EwaJacobian ewa_jacobian(const Args& a, const float3& mean, const float* view) {
+    EwaJacobian e;
     float3 t = xform4x3(mean, view);
-    const float limx = 1.3f * tan_fovx;
-    const float limy = 1.3f * tan_fovy;
+    const float limx = 1.3f * a.tan_fovx;
+    const float limy = 1.3f * a.tan_fovy;
     const float txtz = t.x / t.z;
     const float tytz = t.y / t.z;
     t.x = min(limx, max(-limx, txtz)) * t.z;
     t.y = min(limy, max(-limy, tytz)) * t.z;
-    M3 J = m3(focal_x / t.z, 0.0f, -(focal_x * t.x) / (t.z * t.z), 0.0f, focal_y / t.z,
-              -(focal_y * t.y) / (t.z * t.z), 0.f, 0.f, 0.f);
-    M3 W = m3(view[0], view[4], view[8], view[1], view[5], view[9], view[2], view[6], view[10]);
-    M3 T = m3_mul(W, J);
-    M3 Vrk = m3(cov3D[0], cov3D[1], cov3D[2], cov3D[1], cov3D[3], cov3D[4], cov3D[2], cov3D[4],
-                cov3D[5]);
-    M3 cov = m3_mul(m3_mul(m3_t(T), m3_t(Vrk)), T);
+    e.t = t;
+    e.x_grad_mul = txtz < -limx || txtz > limx ? 0.f : 1.f;
+    e.y_grad_mul = tytz < -limy || tytz > limy ? 0.f : 1.f;
+    e.J = m3(a.focal_x / t.z, 0.0f, -(a.focal_x * t.x) / (t.z * t.z), 0.0f, a.focal_y / t.z,
+             -(a.focal_y * t.y) / (t.z * t.z), 0.f, 0.f, 0.f);
+    e.W = m3(view[0], view[4], view[8], view[1], view[5], view[9], view[2], view[6], view[10]);
+    e.T = m3_mul(e.W, e.J);
+    return e;
+}
+
+__device__ __forceinline__ M3 vrk_of(const float* cov3D) {
+    return m3(cov3D[0], cov3D[1], cov3D[2], cov3D[1], cov3D[3], cov3D[4], cov3D[2], cov3D[4], cov3D[5]);
+}
+
+// forward.cu:74-113
+template <class Args>
+__device__ __forceinline__ float3 cov2d_ewa(const Args& a, const float3& mean, const float* cov3D, const float* view) {
+    const M3 T = ewa_jacobian(a, mean, view).T;
+    M3 cov = m3_mul(m3_mul(m3_t(T), m3_t(vrk_of(cov3D))), T);
     cov.c[0][0] += 0.3f;
     cov.c[1][1] += 0.3f;
     return {cov.c[0][0], cov.c[0][1], cov.c[1][1]};
+}
+
+// conic -> cov2D -> T and t (backward.cu:144-264): the gradients of the loss with respect to cov2D's entries a, b, c
+// (zero unless nonsingular, i.e. denom2inv != 0), to dL/d(W J)[k][j] = dL_dT[k][j] and to the clamped camera-space
+// mean t (the depth term excluded).  dL_dconic = {x, y, z} of the conic {a', b', c'}.
+struct Cov2dGrad {
+    float dL_da, dL_db, dL_dc;
+    bool nonsingular;
+    float dL_dT[2][3];
+    float3 dL_dt;
+};
+template <class Args>
+__device__ __forceinline__ Cov2dGrad cov2d_backward(const Args& a, const EwaJacobian& e, const float* cov3D,
+                                                    float3 dL_dconic) {
+    Cov2dGrad g;
+    const float h_x = a.focal_x, h_y = a.focal_y;
+    const M3& T = e.T;
+    const M3& W = e.W;
+    const M3 Vrk = vrk_of(cov3D);
+    const M3 cov2D = m3_mul(m3_mul(m3_t(T), m3_t(Vrk)), T);
+    const float ca = cov2D.c[0][0] + 0.3f;
+    const float cb = cov2D.c[0][1];
+    const float cc = cov2D.c[1][1] + 0.3f;
+    const float denom = ca * cc - cb * cb;
+    float dL_da = 0, dL_db = 0, dL_dc = 0;
+    const float denom2inv = 1.0f / ((denom * denom) + 0.0000001f);
+    g.nonsingular = denom2inv != 0;
+    if (g.nonsingular) {
+        dL_da = denom2inv * (-cc * cc * dL_dconic.x + 2 * cb * cc * dL_dconic.y + (denom - ca * cc) * dL_dconic.z);
+        dL_dc = denom2inv * (-ca * ca * dL_dconic.z + 2 * ca * cb * dL_dconic.y + (denom - ca * cc) * dL_dconic.x);
+        dL_db = denom2inv * 2 * (cb * cc * dL_dconic.x - (denom + 2 * cb * cb) * dL_dconic.y + ca * cb * dL_dconic.z);
+    }
+    g.dL_da = dL_da;
+    g.dL_db = dL_db;
+    g.dL_dc = dL_dc;
+    // dL_dT[k][j] = 2 (row k of T . column j of Vrk) dL_d(a or c) + (the other row . column j) dL_db
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            const float own = T.c[k][0] * Vrk.c[j][0] + T.c[k][1] * Vrk.c[j][1] + T.c[k][2] * Vrk.c[j][2];
+            const float other = T.c[1 - k][0] * Vrk.c[j][0] + T.c[1 - k][1] * Vrk.c[j][1] + T.c[1 - k][2] * Vrk.c[j][2];
+            g.dL_dT[k][j] = 2 * own * (k == 0 ? dL_da : dL_dc) + other * dL_db;
+        }
+    const float (&dT)[2][3] = g.dL_dT;
+    const float dL_dJ00 = W.c[0][0] * dT[0][0] + W.c[0][1] * dT[0][1] + W.c[0][2] * dT[0][2];
+    const float dL_dJ02 = W.c[2][0] * dT[0][0] + W.c[2][1] * dT[0][1] + W.c[2][2] * dT[0][2];
+    const float dL_dJ11 = W.c[1][0] * dT[1][0] + W.c[1][1] * dT[1][1] + W.c[1][2] * dT[1][2];
+    const float dL_dJ12 = W.c[2][0] * dT[1][0] + W.c[2][1] * dT[1][1] + W.c[2][2] * dT[1][2];
+    const float3 t = e.t;
+    const float tz = 1.f / t.z;
+    const float tz2 = tz * tz;
+    const float tz3 = tz2 * tz;
+    g.dL_dt.x = e.x_grad_mul * -h_x * tz2 * dL_dJ02;
+    g.dL_dt.y = e.y_grad_mul * -h_y * tz2 * dL_dJ12;
+    g.dL_dt.z = -h_x * tz2 * dL_dJ00 - h_y * tz2 * dL_dJ11 + (2 * h_x * t.x) * tz3 * dL_dJ02 +
+                (2 * h_y * t.y) * tz3 * dL_dJ12;
+    return g;
 }
 
 // forward.cu:20-71. sh points at this Gaussian's M coefficients ([M][3]).
@@ -186,6 +279,46 @@ __device__ __forceinline__ float3 sh_to_rgb(int deg, const float3 pos, const flo
     }
     clamped = (uint8_t)((res[0] < 0 ? 1 : 0) | (res[1] < 0 ? 2 : 0) | (res[2] < 0 ? 4 : 0));
     return {fmaxf(res[0], 0.0f), fmaxf(res[1], 0.0f), fmaxf(res[2], 0.0f)};
+}
+
+// dL/d(normalised dir) of the SH colour, summed over the channels (backward.cu:20-139).  (x, y, z): the normalised
+// direction, sh: the Gaussian's [M][3] coefficients, dRGB: dL/dcolour with the clamped channels zeroed.
+__device__ __forceinline__ float3 sh_ddir(int deg, float x, float y, float z, const float* sh, const float dRGB[3]) {
+    float ddir[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+#define SH(i) sh[(i) * 3 + c]
+        float dx_ = 0.f, dy_ = 0.f, dz_ = 0.f;
+        if (deg > 0) {
+            dx_ = -kC1 * SH(3);
+            dy_ = -kC1 * SH(1);
+            dz_ = kC1 * SH(2);
+            if (deg > 1) {
+                dx_ += kC2[0] * y * SH(4) + kC2[2] * 2.f * -x * SH(6) + kC2[3] * z * SH(7) + kC2[4] * 2.f * x * SH(8);
+                dy_ += kC2[0] * x * SH(4) + kC2[1] * z * SH(5) + kC2[2] * 2.f * -y * SH(6) + kC2[4] * 2.f * -y * SH(8);
+                dz_ += kC2[1] * y * SH(5) + kC2[2] * 2.f * 2.f * z * SH(6) + kC2[3] * x * SH(7);
+                if (deg > 2) {
+                    float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+                    dx_ += (kC3[0] * SH(9) * 3.f * 2.f * xy + kC3[1] * SH(10) * yz +
+                            kC3[2] * SH(11) * -2.f * xy + kC3[3] * SH(12) * -3.f * 2.f * xz +
+                            kC3[4] * SH(13) * (-3.f * xx + 4.f * zz - yy) +
+                            kC3[5] * SH(14) * 2.f * xz + kC3[6] * SH(15) * 3.f * (xx - yy));
+                    dy_ += (kC3[0] * SH(9) * 3.f * (xx - yy) + kC3[1] * SH(10) * xz +
+                            kC3[2] * SH(11) * (-3.f * yy + 4.f * zz - xx) +
+                            kC3[3] * SH(12) * -3.f * 2.f * yz + kC3[4] * SH(13) * -2.f * xy +
+                            kC3[5] * SH(14) * -2.f * yz + kC3[6] * SH(15) * -3.f * 2.f * xy);
+                    dz_ += (kC3[1] * SH(10) * xy + kC3[2] * SH(11) * 4.f * 2.f * yz +
+                            kC3[3] * SH(12) * 3.f * (2.f * zz - xx - yy) +
+                            kC3[4] * SH(13) * 4.f * 2.f * xz + kC3[5] * SH(14) * (xx - yy));
+                }
+            }
+        }
+#undef SH
+        ddir[0] += dx_ * dRGB[c];
+        ddir[1] += dy_ * dRGB[c];
+        ddir[2] += dz_ * dRGB[c];
+    }
+    return make_float3(ddir[0], ddir[1], ddir[2]);
 }
 
 struct PreFwdArgs {
@@ -310,16 +443,10 @@ __device__ __forceinline__ bool project_gaussian(const PreFwdArgs& a, const Cam&
     const float3 p_proj = {p_hom.x * p_w, p_hom.y * p_w, p_hom.z * p_w};
 
     float cov3D[6];
-    if (a.cov3D_precomp != nullptr) {
-#pragma unroll
-        for (int i = 0; i < 6; ++i) cov3D[i] = a.cov3D_precomp[6 * idx + i];
-    } else {
-        const float3 s = {a.scales[3 * idx], a.scales[3 * idx + 1], a.scales[3 * idx + 2]};
-        const float4 q = reinterpret_cast<const float4*>(a.rotations)[idx];
-        cov3d_from_scale_rot(s, a.scale_modifier, q, cov3D);
-    }
-    const float3 cov =
-        cov2d_ewa(p_orig, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy, cov3D, cam.view);
+    float3 scl;
+    float4 rot;
+    load_cov3d(a, idx, cov3D, scl, rot);
+    const float3 cov = cov2d_ewa(a, p_orig, cov3D, cam.view);
 
     const float det = (cov.x * cov.z - cov.y * cov.y);
     if (det == 0.0f) return false;
@@ -555,49 +682,16 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(con
     } else {
         const float3 mean = {a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2]};
         float cov3D[6];
-        float3 scl = {0.f, 0.f, 0.f};
-        float4 rot = {0.f, 0.f, 0.f, 0.f};
-        if (a.cov3D_precomp) {
-#pragma unroll
-            for (int i = 0; i < 6; ++i) cov3D[i] = a.cov3D_precomp[6 * idx + i];
-        } else {
-            scl = {a.scales[3 * idx], a.scales[3 * idx + 1], a.scales[3 * idx + 2]};
-            rot = reinterpret_cast<const float4*>(a.rotations)[idx];
-            cov3d_from_scale_rot(scl, a.scale_modifier, rot, cov3D);
-        }
+        float3 scl;
+        float4 rot;
+        load_cov3d(a, idx, cov3D, scl, rot);
         // ---- conic -> cov2D -> cov3D, mean (backward.cu:144-274) ----------
         {
-            const float3 dL_dconic = {g[2], g[3], g[4]};
-            float3 t = xform4x3(mean, view);
-            const float limx = 1.3f * a.tan_fovx, limy = 1.3f * a.tan_fovy;
-            const float txtz = t.x / t.z, tytz = t.y / t.z;
-            t.x = min(limx, max(-limx, txtz)) * t.z;
-            t.y = min(limy, max(-limy, tytz)) * t.z;
-            const float x_grad_mul = txtz < -limx || txtz > limx ? 0.f : 1.f;
-            const float y_grad_mul = tytz < -limy || tytz > limy ? 0.f : 1.f;
-            const float h_x = a.focal_x, h_y = a.focal_y;
-            M3 J = m3(h_x / t.z, 0.0f, -(h_x * t.x) / (t.z * t.z), 0.0f, h_y / t.z,
-                      -(h_y * t.y) / (t.z * t.z), 0.f, 0.f, 0.f);
-            M3 W = m3(view[0], view[4], view[8], view[1], view[5], view[9], view[2], view[6],
-                      view[10]);
-            M3 Vrk = m3(cov3D[0], cov3D[1], cov3D[2], cov3D[1], cov3D[3], cov3D[4], cov3D[2],
-                        cov3D[4], cov3D[5]);
-            M3 T = m3_mul(W, J);
-            M3 cov2D = m3_mul(m3_mul(m3_t(T), m3_t(Vrk)), T);
-            const float ca = cov2D.c[0][0] + 0.3f;
-            const float cb = cov2D.c[0][1];
-            const float cc = cov2D.c[1][1] + 0.3f;
-            const float denom = ca * cc - cb * cb;
-            float dL_da = 0, dL_db = 0, dL_dc = 0;
-            const float denom2inv = 1.0f / ((denom * denom) + 0.0000001f);
-            if (denom2inv != 0) {
-                dL_da = denom2inv * (-cc * cc * dL_dconic.x + 2 * cb * cc * dL_dconic.y +
-                                     (denom - ca * cc) * dL_dconic.z);
-                dL_dc = denom2inv * (-ca * ca * dL_dconic.z + 2 * ca * cb * dL_dconic.y +
-                                     (denom - ca * cc) * dL_dconic.x);
-                dL_db = denom2inv * 2 *
-                        (cb * cc * dL_dconic.x - (denom + 2 * cb * cb) * dL_dconic.y +
-                         ca * cb * dL_dconic.z);
+            const EwaJacobian e = ewa_jacobian(a, mean, view);
+            const Cov2dGrad cg = cov2d_backward(a, e, cov3D, make_float3(g[2], g[3], g[4]));
+            if (cg.nonsingular) {
+                const M3& T = e.T;
+                const float dL_da = cg.dL_da, dL_db = cg.dL_db, dL_dc = cg.dL_dc;
                 dcov[0] = (T.c[0][0] * T.c[0][0] * dL_da + T.c[0][0] * T.c[1][0] * dL_db +
                            T.c[1][0] * T.c[1][0] * dL_dc);
                 dcov[3] = (T.c[0][1] * T.c[0][1] * dL_da + T.c[0][1] * T.c[1][1] * dL_db +
@@ -614,33 +708,11 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(con
                           (T.c[0][1] * T.c[1][2] + T.c[0][2] * T.c[1][1]) * dL_db +
                           2 * T.c[1][1] * T.c[1][2] * dL_dc;
             }
-            const float dL_dT00 = 2 * (T.c[0][0] * Vrk.c[0][0] + T.c[0][1] * Vrk.c[0][1] + T.c[0][2] * Vrk.c[0][2]) * dL_da +
-                                  (T.c[1][0] * Vrk.c[0][0] + T.c[1][1] * Vrk.c[0][1] + T.c[1][2] * Vrk.c[0][2]) * dL_db;
-            const float dL_dT01 = 2 * (T.c[0][0] * Vrk.c[1][0] + T.c[0][1] * Vrk.c[1][1] + T.c[0][2] * Vrk.c[1][2]) * dL_da +
-                                  (T.c[1][0] * Vrk.c[1][0] + T.c[1][1] * Vrk.c[1][1] + T.c[1][2] * Vrk.c[1][2]) * dL_db;
-            const float dL_dT02 = 2 * (T.c[0][0] * Vrk.c[2][0] + T.c[0][1] * Vrk.c[2][1] + T.c[0][2] * Vrk.c[2][2]) * dL_da +
-                                  (T.c[1][0] * Vrk.c[2][0] + T.c[1][1] * Vrk.c[2][1] + T.c[1][2] * Vrk.c[2][2]) * dL_db;
-            const float dL_dT10 = 2 * (T.c[1][0] * Vrk.c[0][0] + T.c[1][1] * Vrk.c[0][1] + T.c[1][2] * Vrk.c[0][2]) * dL_dc +
-                                  (T.c[0][0] * Vrk.c[0][0] + T.c[0][1] * Vrk.c[0][1] + T.c[0][2] * Vrk.c[0][2]) * dL_db;
-            const float dL_dT11 = 2 * (T.c[1][0] * Vrk.c[1][0] + T.c[1][1] * Vrk.c[1][1] + T.c[1][2] * Vrk.c[1][2]) * dL_dc +
-                                  (T.c[0][0] * Vrk.c[1][0] + T.c[0][1] * Vrk.c[1][1] + T.c[0][2] * Vrk.c[1][2]) * dL_db;
-            const float dL_dT12 = 2 * (T.c[1][0] * Vrk.c[2][0] + T.c[1][1] * Vrk.c[2][1] + T.c[1][2] * Vrk.c[2][2]) * dL_dc +
-                                  (T.c[0][0] * Vrk.c[2][0] + T.c[0][1] * Vrk.c[2][1] + T.c[0][2] * Vrk.c[2][2]) * dL_db;
-            const float dL_dJ00 = W.c[0][0] * dL_dT00 + W.c[0][1] * dL_dT01 + W.c[0][2] * dL_dT02;
-            const float dL_dJ02 = W.c[2][0] * dL_dT00 + W.c[2][1] * dL_dT01 + W.c[2][2] * dL_dT02;
-            const float dL_dJ11 = W.c[1][0] * dL_dT10 + W.c[1][1] * dL_dT11 + W.c[1][2] * dL_dT12;
-            const float dL_dJ12 = W.c[2][0] * dL_dT10 + W.c[2][1] * dL_dT11 + W.c[2][2] * dL_dT12;
-            const float tz = 1.f / t.z;
-            const float tz2 = tz * tz;
-            const float tz3 = tz2 * tz;
-            const float dL_dtx = x_grad_mul * -h_x * tz2 * dL_dJ02;
-            const float dL_dty = y_grad_mul * -h_y * tz2 * dL_dJ12;
-            const float dL_dtz = -h_x * tz2 * dL_dJ00 - h_y * tz2 * dL_dJ11 +
-                                 (2 * h_x * t.x) * tz3 * dL_dJ02 + (2 * h_y * t.y) * tz3 * dL_dJ12;
             // transformVec4x3Transpose (auxiliary.h:89-97); assignment, backward.cu:273
-            dmean[0] = view[0] * dL_dtx + view[1] * dL_dty + view[2] * dL_dtz;
-            dmean[1] = view[4] * dL_dtx + view[5] * dL_dty + view[6] * dL_dtz;
-            dmean[2] = view[8] * dL_dtx + view[9] * dL_dty + view[10] * dL_dtz;
+            const float3 dt = cg.dL_dt;
+            dmean[0] = view[0] * dt.x + view[1] * dt.y + view[2] * dt.z;
+            dmean[1] = view[4] * dt.x + view[5] * dt.y + view[6] * dt.z;
+            dmean[2] = view[8] * dt.x + view[9] * dt.y + view[10] * dt.z;
         }
         // ---- screen-space mean and depth terms (backward.cu:372-403) ------
         {
@@ -668,8 +740,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(con
             const float len = sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
             const float x = dir_orig.x / len, y = dir_orig.y / len, z = dir_orig.z / len;
             const uint8_t cl = a.clamped[idx];
-            float dRGB[3] = {(cl & 1) ? 0.f : g[6], (cl & 2) ? 0.f : g[7], (cl & 4) ? 0.f : g[8]};
-            float ddir[3] = {0.f, 0.f, 0.f};   // dL/ddir
+            const float dRGB[3] = {(cl & 1) ? 0.f : g[6], (cl & 2) ? 0.f : g[7], (cl & 4) ? 0.f : g[8]};
             const int deg = a.D;
             float basis[16];
             basis[0] = kC0;
@@ -695,40 +766,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(con
                     }
                 }
             }
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-#define SH(i) sh[(i) * 3 + c]
-                float dx_ = 0.f, dy_ = 0.f, dz_ = 0.f;
-                if (deg > 0) {
-                    dx_ = -kC1 * SH(3);
-                    dy_ = -kC1 * SH(1);
-                    dz_ = kC1 * SH(2);
-                    if (deg > 1) {
-                        dx_ += kC2[0] * y * SH(4) + kC2[2] * 2.f * -x * SH(6) + kC2[3] * z * SH(7) + kC2[4] * 2.f * x * SH(8);
-                        dy_ += kC2[0] * x * SH(4) + kC2[1] * z * SH(5) + kC2[2] * 2.f * -y * SH(6) + kC2[4] * 2.f * -y * SH(8);
-                        dz_ += kC2[1] * y * SH(5) + kC2[2] * 2.f * 2.f * z * SH(6) + kC2[3] * x * SH(7);
-                        if (deg > 2) {
-                            float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-                            dx_ += (kC3[0] * SH(9) * 3.f * 2.f * xy + kC3[1] * SH(10) * yz +
-                                    kC3[2] * SH(11) * -2.f * xy + kC3[3] * SH(12) * -3.f * 2.f * xz +
-                                    kC3[4] * SH(13) * (-3.f * xx + 4.f * zz - yy) +
-                                    kC3[5] * SH(14) * 2.f * xz + kC3[6] * SH(15) * 3.f * (xx - yy));
-                            dy_ += (kC3[0] * SH(9) * 3.f * (xx - yy) + kC3[1] * SH(10) * xz +
-                                    kC3[2] * SH(11) * (-3.f * yy + 4.f * zz - xx) +
-                                    kC3[3] * SH(12) * -3.f * 2.f * yz + kC3[4] * SH(13) * -2.f * xy +
-                                    kC3[5] * SH(14) * -2.f * yz + kC3[6] * SH(15) * -3.f * 2.f * xy);
-                            dz_ += (kC3[1] * SH(10) * xy + kC3[2] * SH(11) * 4.f * 2.f * yz +
-                                    kC3[3] * SH(12) * 3.f * (2.f * zz - xx - yy) +
-                                    kC3[4] * SH(13) * 4.f * 2.f * xz + kC3[5] * SH(14) * (xx - yy));
-                        }
-                    }
-                }
-#undef SH
-                ddir[0] += dx_ * dRGB[c];
-                ddir[1] += dy_ * dRGB[c];
-                ddir[2] += dz_ * dRGB[c];
-            }
-            const float3 dm = dnormvdv3(dir_orig, make_float3(ddir[0], ddir[1], ddir[2]));
+            const float3 dm = dnormvdv3(dir_orig, sh_ddir(deg, x, y, z, sh, dRGB));
             dmean[0] += dm.x; dmean[1] += dm.y; dmean[2] += dm.z;
             // all reads of this lane's coefficients are done: the row now carries dL/dsh
             for (int i = 0; i < Msh; ++i) {
