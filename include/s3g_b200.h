@@ -264,6 +264,28 @@ int s3g_rasterize_backward_opacity(const s3g_raster_scene* scene, const s3g_rast
 int s3g_rasterize_backward_deterministic_opacity(const s3g_raster_scene* scene, const s3g_raster_backward_args* bwd,
                                                  const s3g_raster_opacity_args* opa, void* workspace, void* stream);
 
+/* ---- antialiasing (Mip-Splatting's 2-D screen-space filter) --------------------------------------------------------
+ * Not in the reference rasterizer; upstream 3DGS calls it `antialiasing`, gsplat rasterize_mode="antialiased".  Every
+ * Gaussian's 2-D covariance is dilated by 0.3 px^2, so one smaller than a pixel is drawn as a blob of at least that
+ * size and grows brighter and thicker as the pixels grow (a model rendered below its training resolution, distant
+ * geometry).  The antialiased forward keeps that dilation and scales the opacity by the ratio of the footprints:
+ *   with a, b, c the EWA 2-D covariance before the dilation, det0 = a c - b^2, det1 = (a + 0.3)(c + 0.3) - b^2,
+ *   h = sqrt(max(det0 / det1, 2.5e-5)), the composite uses alpha_eff = opacity * h wherever it reads an opacity (the
+ *   blend weight, the 1/255 cut-off, the tile culling, the alpha and median images).
+ * Conic, radii, tile rectangles and depth keys are those of the plain forward.
+ * s3g_rasterize_forward_antialiased is s3g_rasterize_forward_opacity (so, with a NULL `opa` or every field NULL,
+ * s3g_rasterize_forward) with the filter on: the same scene, arguments, contract and extras (aux pair, decomposition,
+ * flow sets, opacity images).  The choice is made once, at the forward: the library remembers per geometry buffer
+ * whether its last forward was antialiased (every forward updates that record), and s3g_rasterize_backward, its
+ * deterministic and *_opacity forms and s3g_rasterize_camera_backward then apply that forward's chain rule: dL_dopacity
+ * is h dL/dalpha_eff, and the term of h's dependence on the 2-D covariance reaches dL_dmean3D, dL_dscale, dL_drot,
+ * dL_dcov3D and the camera gradients (dL_dmean2D, dL_dconic and dL_ddepth are the composite's, as before).  They read
+ * the record through bwd->geom_buffer, so the camera pass needs it after an antialiased forward.
+ * S3G_ERR_ARG before any launch: every case of s3g_rasterize_forward_opacity; in a backward, a peer sink after an
+ * antialiased forward (the fused gradient exchange does not take its gradients). */
+int64_t s3g_rasterize_forward_antialiased(const s3g_raster_scene* scene, const s3g_raster_forward_args* fwd,
+                                          const s3g_raster_opacity_args* opa /* may be NULL */, void* stream);
+
 /* ---- camera gradients ---------------------------------------------------------------------------------------------
  * Extends the backward of _RasterizeGaussians (DGR/diff_gaussian_rasterization/__init__.py:101-156), which returns no
  * gradient for raster_settings, and Rasterizer::backward (rasterizer.h:58-88): the gradient of the same loss with

@@ -34,6 +34,8 @@ SIGNATURES = {
     "s3g_rasterize_forward_opacity": (_I64, [_V, _V, _V, _V]),
     "s3g_rasterize_backward_opacity": (_I, [_V, _V, _V, _V]),
     "s3g_rasterize_backward_deterministic_opacity": (_I, [_V, _V, _V, _V, _V]),
+    # s3g_rasterize_forward_opacity with the antialiasing filter; the RasterOpacityArgs may be NULL
+    "s3g_rasterize_forward_antialiased": (_I64, [_V, _V, _V, _V]),
     # s3g_rasterize_camera_backward also takes a RasterCameraGrads (below) with ctypes.byref()
     "s3g_rasterize_camera_backward_workspace_bytes": (_SZ, [_I]),
     "s3g_rasterize_camera_backward": (_I, [_V, _V, _V, _V, _V]),

@@ -12,6 +12,7 @@
 #include <cstring>
 #include <mutex>
 #include <string>
+#include <unordered_set>
 #include <vector>
 
 #include "api_common.cuh"
@@ -293,6 +294,24 @@ bool has_median_state(const char* image, int width, int height) {
     return false;
 }
 
+// Geometry buffers whose last forward was antialiased (s3g_rasterize_forward_antialiased): the backward and the camera
+// pass apply that forward's chain rule, chosen on the host before any launch.  Every forward on a buffer updates its
+// entry.  Unlike the median record this one has no cap: a forgotten entry would silently give the plain gradients.
+// It holds one pointer per distinct buffer address an antialiased forward has used and no later forward has reused.
+std::mutex g_aa_mu;
+std::unordered_set<const char*> g_aa_states;
+
+void note_aa_state(const char* geom, bool antialiased) {
+    std::lock_guard<std::mutex> lock(g_aa_mu);
+    if (antialiased) g_aa_states.insert(geom);
+    else g_aa_states.erase(geom);
+}
+bool has_aa_state(const char* geom) {
+    if (!geom) return false;
+    std::lock_guard<std::mutex> lock(g_aa_mu);
+    return g_aa_states.count(geom) != 0;
+}
+
 // one forward composite walk; the plain walks take the RenderFwdArgs part of ra, and an opacity walk is launched when
 // opa is given
 template <int NA, bool SPLIT>
@@ -302,9 +321,9 @@ void launch_render_forward(const RenderSplitArgs& ra, const AuxSet& a1, const Op
     else render_forward_kernel<NA, SPLIT><<<grid, TILE_PIX, 0, stream>>>(ra, a1);
 }
 
-// o: the opacity outputs (s3g_rasterize_forward_opacity), or NULL for the plain forward
+// o: the opacity outputs (s3g_rasterize_forward_opacity), or NULL for the plain forward.  aa: antialiased
 int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f, const s3g_raster_opacity_args* o,
-                     cudaStream_t stream) {
+                     bool aa, cudaStream_t stream) {
     const int P = s.P, width = s.width, height = s.height, debug = s.debug;
     if (P < 0 || width <= 0 || height <= 0) return fail(S3G_ERR_ARG, "forward: bad sizes");
     if (!f.geom_alloc || !f.binning_alloc || !f.image_alloc) return fail(S3G_ERR_ARG, "forward: null allocator");
@@ -379,6 +398,7 @@ int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f
     char* gptr = f.geom_alloc(f.geom_user, s3g_geom_bytes(P));
     if (!gptr) return fail(S3G_ERR_ALLOC, "forward: geometry allocator returned NULL");
     GeomState geom = GeomState::carve(gptr, P);
+    note_aa_state(gptr, aa);
     char* iptr = f.image_alloc(f.image_user, s3g_image_bytes(width, height));
     if (!iptr) return fail(S3G_ERR_ALLOC, "forward: image allocator returned NULL");
     ImageState img = ImageState::carve(iptr, width, height);
@@ -410,9 +430,12 @@ int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f
     S3G_CUDA(cudaMemsetAsync(geom.scan_status, 0, geom.zero_bytes, stream), "memset scan/sort state");
     S3G_MARK(0, "preprocess_forward");
     {
-        const int rc = launch_sh_rows(preprocess_forward_kernel<16>, preprocess_forward_kernel<0>, pa,
-                                      (P + PRE_THREADS - 1) / PRE_THREADS, PRE_THREADS, s.M,
-                                      s.colors_precomp == nullptr, "forward", stream);
+        const int grid = (P + PRE_THREADS - 1) / PRE_THREADS;
+        const bool use_sh = s.colors_precomp == nullptr;
+        const int rc = aa ? launch_sh_rows(preprocess_forward_kernel<16, true>, preprocess_forward_kernel<0, true>, pa,
+                                           grid, PRE_THREADS, s.M, use_sh, "forward", stream)
+                          : launch_sh_rows(preprocess_forward_kernel<16>, preprocess_forward_kernel<0>, pa, grid,
+                                           PRE_THREADS, s.M, use_sh, "forward", stream);
         if (rc != S3G_OK) return rc;
     }
     S3G_STAGE("preprocess_forward");
@@ -604,6 +627,10 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
         for (int p = 0; p < sink->world; ++p)
             if (!sink->stage[p]) return fail(S3G_ERR_ARG, "backward_dp: null staging pointer");
     }
+    const bool aa = has_aa_state(b.geom_buffer);
+    if (sink && aa)
+        return fail(S3G_ERR_ARG, "backward_dp: the fused gradient exchange does not take an antialiased forward's "
+                                 "gradients");
     if ((b.dL_dpix_aux != nullptr) != (b.dL_dcolor_aux != nullptr))
         return fail(S3G_ERR_ARG, "backward: dL_dpix_aux and dL_dcolor_aux go together");
     const bool use_aux = b.dL_dpix_aux != nullptr;
@@ -689,6 +716,7 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
     pb.dL_dcolor = b.dL_dcolor; pb.dL_dcolor_aux = b.dL_dcolor_aux; pb.dL_ddepth = b.dL_ddepth; pb.dL_dmean3D = b.dL_dmean3D;
     pb.dL_dcov3D = b.dL_dcov3D; pb.dL_dsh = use_sh ? b.dL_dsh : nullptr;
     pb.dL_dscale = b.dL_dscale; pb.dL_drot = b.dL_drot;
+    pb.Cod = geom.Cod;
     if (sink) {
         for (int p = 0; p < 16; ++p) pb.sink.stage[p] = p < sink->world ? static_cast<float*>(sink->stage[p]) : nullptr;
         pb.sink.world = sink->world; pb.sink.rank = sink->rank; pb.sink.chunk = sink->chunk;
@@ -699,6 +727,9 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
         const int grid = (P + PRE_THREADS - 1) / PRE_THREADS;
         const int rc = sink ? launch_sh_rows(preprocess_backward_kernel<16, true>, preprocess_backward_kernel<0, true>,
                                              pb, grid, PRE_THREADS, s.M, use_sh, "backward", stream)
+                       : aa ? launch_sh_rows(preprocess_backward_kernel<16, false, true>,
+                                             preprocess_backward_kernel<0, false, true>, pb, grid, PRE_THREADS, s.M,
+                                             use_sh, "backward", stream)
                             : launch_sh_rows(preprocess_backward_kernel<16>, preprocess_backward_kernel<0>, pb, grid,
                                              PRE_THREADS, s.M, use_sh, "backward", stream);
         if (rc != S3G_OK) return rc;
@@ -713,13 +744,19 @@ extern "C" {
 
 int64_t s3g_rasterize_forward(const s3g_raster_scene* scene, const s3g_raster_forward_args* fwd, void* stream) {
     if (!scene || !fwd) return fail(S3G_ERR_ARG, "forward: null scene / forward arguments");
-    return forward_impl(*scene, *fwd, nullptr, static_cast<cudaStream_t>(stream));
+    return forward_impl(*scene, *fwd, nullptr, false, static_cast<cudaStream_t>(stream));
 }
 
 int64_t s3g_rasterize_forward_opacity(const s3g_raster_scene* scene, const s3g_raster_forward_args* fwd,
                                       const s3g_raster_opacity_args* opa, void* stream) {
     if (!scene || !fwd) return fail(S3G_ERR_ARG, "forward_opacity: null scene / forward arguments");
-    return forward_impl(*scene, *fwd, opa, static_cast<cudaStream_t>(stream));
+    return forward_impl(*scene, *fwd, opa, false, static_cast<cudaStream_t>(stream));
+}
+
+int64_t s3g_rasterize_forward_antialiased(const s3g_raster_scene* scene, const s3g_raster_forward_args* fwd,
+                                          const s3g_raster_opacity_args* opa, void* stream) {
+    if (!scene || !fwd) return fail(S3G_ERR_ARG, "forward_antialiased: null scene / forward arguments");
+    return forward_impl(*scene, *fwd, opa, true, static_cast<cudaStream_t>(stream));
 }
 
 int s3g_rasterize_backward(const s3g_raster_scene* scene, const s3g_raster_backward_args* bwd, void* stream) {
@@ -802,10 +839,18 @@ int s3g_rasterize_camera_backward(const s3g_raster_scene* scene, const s3g_raste
     ca.dL_dmean2D = b.dL_dmean2D; ca.dL_dconic = b.dL_dconic; ca.dL_ddepth = b.dL_ddepth; ca.dL_dcolor = b.dL_dcolor;
     ca.partial = static_cast<double*>(workspace);
     ca.nblocks = camera_grad_blocks(P);
+    // after an antialiased forward: the opacity factor's term, from the records that forward and the backward left
+    const bool aa = has_aa_state(b.geom_buffer);
+    ca.grad_rec = geom.grad_rec; ca.Cod = geom.Cod;
     if (campos) {
-        const int rc = launch_sh_rows(camera_grad_partial_kernel<16, true>, camera_grad_partial_kernel<0, true>, ca,
-                                      ca.nblocks, CAM_THREADS, s.M, true, "camera_backward", stream);
+        const int rc = aa ? launch_sh_rows(camera_grad_partial_kernel<16, true, true>,
+                                           camera_grad_partial_kernel<0, true, true>, ca, ca.nblocks, CAM_THREADS,
+                                           s.M, true, "camera_backward", stream)
+                          : launch_sh_rows(camera_grad_partial_kernel<16, true>, camera_grad_partial_kernel<0, true>,
+                                           ca, ca.nblocks, CAM_THREADS, s.M, true, "camera_backward", stream);
         if (rc != S3G_OK) return rc;
+    } else if (aa) {
+        camera_grad_partial_kernel<0, false, true><<<ca.nblocks, CAM_THREADS, 0, stream>>>(ca);
     } else {
         camera_grad_partial_kernel<0, false><<<ca.nblocks, CAM_THREADS, 0, stream>>>(ca);
     }

@@ -50,12 +50,15 @@ struct CamBwdArgs {
     const float* dL_dcolor;    // [P,3]
     double* partial;           // [CAM_NCOMP][nblocks]
     int nblocks;
+    const float* grad_rec;     // AA only: the composite's records, [P][GRAD_REC], slot 5 = dL/dalpha_eff
+    const float4* Cod;         // AA only: the forward's records, .y = alpha_eff
 };
 
 __host__ __device__ inline int camera_grad_blocks(int P) { return (int)div_up64(P, CAM_GAUSS_PER_BLOCK); }
 
 // One visible Gaussian's contribution to the CAM_NCOMP components.  sh: its staged coefficient row when CAMPOS.
-template <bool CAMPOS>
+// AA: after an antialiased forward, whose opacity factor depends on the 2-D covariance and so on the camera.
+template <bool CAMPOS, bool AA>
 __device__ __forceinline__ void camera_contrib(const CamBwdArgs& a, const Cam& cam, int idx, const float* sh,
                                                float c[CAM_NCOMP]) {
     const float* view = cam.view;
@@ -69,7 +72,8 @@ __device__ __forceinline__ void camera_contrib(const CamBwdArgs& a, const Cam& c
 
     // ---- conic -> cov2D -> T = J W and t, as the preprocess backward ------------------------------------------------
     const EwaJacobian e = ewa_jacobian(a, mean, view);
-    const Cov2dGrad g = cov2d_backward(a, e, cov3D, make_float3(dconic.x, dconic.y, dconic.w));
+    const Cov2dGrad g = cov2d_backward<AA>(a, e, cov3D, make_float3(dconic.x, dconic.y, dconic.w),
+                                           AA ? a.Cod[idx].y * a.grad_rec[(size_t)idx * GRAD_REC + 5] : 0.f);
     const M3& J = e.J;
     // dT[k][j] = dL/d(J W)[k][j] (row k of the 2x3 product, column j): T.c[k][j] in the glm layout
     const float (&dT)[2][3] = g.dL_dT;
@@ -114,7 +118,7 @@ __device__ __forceinline__ void camera_contrib(const CamBwdArgs& a, const Cam& c
 }
 
 // Block b sums Gaussians [b * CAM_GAUSS_PER_BLOCK, (b + 1) * CAM_GAUSS_PER_BLOCK) into partial[k][b].
-template <int MT, bool CAMPOS>   // MT = 16: SH rows of 48 floats known at compile time; 0: runtime M
+template <int MT, bool CAMPOS, bool AA = false>   // MT = 16: SH rows of 48 floats known at compile time; 0: runtime M
 __global__ void __launch_bounds__(CAM_THREADS) camera_grad_partial_kernel(const __grid_constant__ CamBwdArgs a) {
     extern __shared__ float s_dyn[];
     __shared__ Cam s_cam;
@@ -137,7 +141,7 @@ __global__ void __launch_bounds__(CAM_THREADS) camera_grad_partial_kernel(const 
         }
         float c[CAM_NCOMP];
         if (visible) {
-            camera_contrib<CAMPOS>(a, s_cam, idx, rows + lane * row_stride(L), c);
+            camera_contrib<CAMPOS, AA>(a, s_cam, idx, rows + lane * row_stride(L), c);
         } else {
 #pragma unroll
             for (int k = 0; k < CAM_NCOMP; ++k) c[k] = 0.f;

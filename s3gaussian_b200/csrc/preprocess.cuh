@@ -175,28 +175,47 @@ __device__ __forceinline__ M3 vrk_of(const float* cov3D) {
     return m3(cov3D[0], cov3D[1], cov3D[2], cov3D[1], cov3D[3], cov3D[4], cov3D[2], cov3D[4], cov3D[5]);
 }
 
-// forward.cu:74-113
+// forward.cu:74-113 without the dilation: the EWA 2-D covariance {a, b, c}
 template <class Args>
-__device__ __forceinline__ float3 cov2d_ewa(const Args& a, const float3& mean, const float* cov3D, const float* view) {
+__device__ __forceinline__ float3 cov2d_ewa_raw(const Args& a, const float3& mean, const float* cov3D,
+                                                const float* view) {
     const M3 T = ewa_jacobian(a, mean, view).T;
-    M3 cov = m3_mul(m3_mul(m3_t(T), m3_t(vrk_of(cov3D))), T);
-    cov.c[0][0] += 0.3f;
-    cov.c[1][1] += 0.3f;
+    const M3 cov = m3_mul(m3_mul(m3_t(T), m3_t(vrk_of(cov3D))), T);
     return {cov.c[0][0], cov.c[0][1], cov.c[1][1]};
 }
+// forward.cu:74-113: the 2-D covariance dilated by 0.3 px^2
+template <class Args>
+__device__ __forceinline__ float3 cov2d_ewa(const Args& a, const float3& mean, const float* cov3D, const float* view) {
+    float3 cov = cov2d_ewa_raw(a, mean, cov3D, view);
+    cov.x += 0.3f;
+    cov.z += 0.3f;
+    return cov;
+}
+
+// Antialiasing (Mip-Splatting's 2-D filter): the dilation by 0.3 px^2 grows a Gaussian's footprint, and with it the
+// energy it puts on screen, the more the smaller it is against a pixel.  The antialiased forms scale its opacity by
+// h = sqrt(max(rho, AA_RHO_MIN)), rho = det0 / det1 the ratio of the 2-D covariance's determinant before and after
+// the dilation, so that the dilated Gaussian carries the energy of the undilated one.  a, b, c: the EWA covariance
+// (cov2d_ewa_raw), det1: the dilated determinant.
+constexpr float AA_RHO_MIN = 2.5e-5f;
+__device__ __forceinline__ float aa_rho(float a, float b, float c, float det1) { return (a * c - b * b) / det1; }
+__device__ __forceinline__ float aa_scale(float rho) { return sqrtf(fmaxf(rho, AA_RHO_MIN)); }
 
 // conic -> cov2D -> T and t (backward.cu:144-264): the gradients of the loss with respect to cov2D's entries a, b, c
 // (zero unless nonsingular, i.e. denom2inv != 0), to dL/d(W J)[k][j] = dL_dT[k][j] and to the clamped camera-space
 // mean t (the depth term excluded).  dL_dconic = {x, y, z} of the conic {a', b', c'}.
+// AA (antialiased forward): alpha_g = dL/dalpha_eff * alpha_eff, with alpha_eff = opacity * h the opacity the
+// composite used; the filter's term dL/drho * drho/d{a, b, c} joins dL_da, dL_db, dL_dc, and aa_h returns h.
 struct Cov2dGrad {
     float dL_da, dL_db, dL_dc;
     bool nonsingular;
     float dL_dT[2][3];
     float3 dL_dt;
+    float aa_h;
 };
-template <class Args>
+template <bool AA = false, class Args>
 __device__ __forceinline__ Cov2dGrad cov2d_backward(const Args& a, const EwaJacobian& e, const float* cov3D,
-                                                    float3 dL_dconic) {
+                                                    float3 dL_dconic, float alpha_g = 0.f) {
     Cov2dGrad g;
     const float h_x = a.focal_x, h_y = a.focal_y;
     const M3& T = e.T;
@@ -214,6 +233,20 @@ __device__ __forceinline__ Cov2dGrad cov2d_backward(const Args& a, const EwaJaco
         dL_da = denom2inv * (-cc * cc * dL_dconic.x + 2 * cb * cc * dL_dconic.y + (denom - ca * cc) * dL_dconic.z);
         dL_dc = denom2inv * (-ca * ca * dL_dconic.z + 2 * ca * cb * dL_dconic.y + (denom - ca * cc) * dL_dconic.x);
         dL_db = denom2inv * 2 * (cb * cc * dL_dconic.x - (denom + 2 * cb * cb) * dL_dconic.y + ca * cb * dL_dconic.z);
+    }
+    if (AA) {
+        const float a0 = cov2D.c[0][0], c0 = cov2D.c[1][1];
+        const float rho = aa_rho(a0, cb, c0, denom);
+        g.aa_h = aa_scale(rho);
+        if (g.nonsingular && rho > AA_RHO_MIN) {
+            // dL/drho = opacity g / (2 h) = alpha_eff g / (2 rho), as h * h = rho here; drho/d{a, b, c} with
+            // det0 = a c - b^2 and det1 = denom = (a + 0.3)(c + 0.3) - b^2
+            const float det0 = a0 * c0 - cb * cb;
+            const float k = alpha_g / (2.f * rho) / (denom * denom);
+            dL_da += k * (c0 * denom - det0 * cc);
+            dL_dc += k * (a0 * denom - det0 * ca);
+            dL_db += k * (-2.f * cb * (0.3f * (a0 + c0) + 0.09f));
+        }
     }
     g.dL_da = dL_da;
     g.dL_db = dL_db;
@@ -429,9 +462,11 @@ struct Projected {
     float3 conic;
     float depth, radius, lam_max, lam_min;
     unsigned rminx, rminy, rmaxx, rmaxy;
+    float aa_h;   // AA: the opacity factor of the antialiasing filter
 };
 
 // Everything of forward.cu:182-237 up to (not including) the colour; false = culled.
+template <bool AA>
 __device__ __forceinline__ bool project_gaussian(const PreFwdArgs& a, const Cam& cam, int idx,
                                                  const float3 p_orig, Projected& o) {
     // near cull (auxiliary.h:152-154)
@@ -446,10 +481,17 @@ __device__ __forceinline__ bool project_gaussian(const PreFwdArgs& a, const Cam&
     float3 scl;
     float4 rot;
     load_cov3d(a, idx, cov3D, scl, rot);
-    const float3 cov = cov2d_ewa(a, p_orig, cov3D, cam.view);
+    float3 raw, cov;
+    if (AA) {
+        raw = cov2d_ewa_raw(a, p_orig, cov3D, cam.view);
+        cov = {raw.x + 0.3f, raw.y, raw.z + 0.3f};
+    } else {
+        cov = cov2d_ewa(a, p_orig, cov3D, cam.view);
+    }
 
     const float det = (cov.x * cov.z - cov.y * cov.y);
     if (det == 0.0f) return false;
+    if (AA) o.aa_h = aa_scale(aa_rho(raw.x, raw.y, raw.z, det));
     const float det_inv = 1.f / det;
     o.conic = {cov.z * det_inv, -cov.y * det_inv, cov.x * det_inv};
 
@@ -475,7 +517,8 @@ __device__ __forceinline__ bool project_gaussian(const PreFwdArgs& a, const Cam&
     return true;
 }
 
-template <int MT>   // MT = 16: SH rows of 48 floats known at compile time; 0: runtime M
+// MT = 16: SH rows of 48 floats known at compile time; 0: runtime M.  AA: the composite gets opacity * h (antialiasing)
+template <int MT, bool AA = false>
 __global__ void __launch_bounds__(PRE_THREADS) preprocess_forward_kernel(PreFwdArgs a) {
     extern __shared__ float s_dyn[];
     __shared__ Cam s_cam;
@@ -493,7 +536,7 @@ __global__ void __launch_bounds__(PRE_THREADS) preprocess_forward_kernel(PreFwdA
         a.depth_key[idx] = DEPTH_KEY_INVISIBLE;
         a.order[idx] = (uint32_t)idx;
         p_orig = {a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2]};
-        vis = project_gaussian(a, s_cam, idx, p_orig, po);
+        vis = project_gaussian<AA>(a, s_cam, idx, p_orig, po);
     }
     uint32_t group_bit = 0;
     if (a.group) {
@@ -519,7 +562,7 @@ __global__ void __launch_bounds__(PRE_THREADS) preprocess_forward_kernel(PreFwdA
         col = {a.colors_precomp[3 * idx], a.colors_precomp[3 * idx + 1], a.colors_precomp[3 * idx + 2]};
     }
     if (!vis) return;
-    const float opacity = a.opacities[idx];
+    const float opacity = AA ? a.opacities[idx] * po.aa_h : a.opacities[idx];
 
     a.clamped[idx] = clamped;
     a.radii[idx] = (int)po.radius;
@@ -597,6 +640,7 @@ struct PreBwdArgs {
     float* dL_dscale;        // [P,3]
     float* dL_drot;          // [P,4]
     PeerSink sink;           // DP kernels only
+    const float4* Cod;       // AA kernels only: the forward's records, .y = the opacity the composite used
 };
 
 __device__ __forceinline__ float3 dnormvdv3(float3 v, float3 dv) {   // auxiliary.h:107-117
@@ -611,8 +655,10 @@ __device__ __forceinline__ float3 dnormvdv3(float3 v, float3 dv) {   // auxiliar
 
 // Register budget capped for 8 resident blocks per SM (64 registers, 20 spilled words): the kernel is HBM-bound and
 // gains from more loads in flight than the unconstrained 96 registers allow.
-template <int MT, bool DP = false>   // MT = 16: compile-time SH row length; 0: runtime M.  DP: gradients go to a.sink
+// MT = 16: compile-time SH row length; 0: runtime M.  DP: gradients go to a.sink.  AA: after an antialiased forward.
+template <int MT, bool DP = false, bool AA = false>
 __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(const __grid_constant__ PreBwdArgs a) {
+    static_assert(!(DP && AA), "the fused gradient exchange does not take the antialiased backward");
     extern __shared__ float s_dyn[];
     __shared__ Cam s_cam;
     load_cam(s_cam, a.view, a.proj, a.campos);
@@ -658,7 +704,8 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(con
         a.dL_dconic[4 * idx + 2] = 0.f;
         a.dL_dconic[4 * idx + 3] = g[4];
     }
-    if (!DP) a.dL_dopacity[idx] = g[5];
+    if (AA) {}   // dL_dopacity = h * g[5] is written below, once h is known
+    else if (!DP) a.dL_dopacity[idx] = g[5];
     else if (visible) *sink_ptr(a.sink, a.sink.off_opacity + idx) = g[5];
     a.dL_dcolor[3 * idx + 0] = g[6];
     a.dL_dcolor[3 * idx + 1] = g[7];
@@ -675,6 +722,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(con
     float dcov[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     float dscale[3] = {0.f, 0.f, 0.f};
     float drot[4] = {0.f, 0.f, 0.f, 0.f};
+    float aa_h = 0.f;
 
     if (!visible) {
         if (a.dL_dsh)
@@ -688,7 +736,9 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(con
         // ---- conic -> cov2D -> cov3D, mean (backward.cu:144-274) ----------
         {
             const EwaJacobian e = ewa_jacobian(a, mean, view);
-            const Cov2dGrad cg = cov2d_backward(a, e, cov3D, make_float3(g[2], g[3], g[4]));
+            const Cov2dGrad cg = cov2d_backward<AA>(a, e, cov3D, make_float3(g[2], g[3], g[4]),
+                                                    AA ? a.Cod[idx].y * g[5] : 0.f);
+            if (AA) aa_h = cg.aa_h;
             if (cg.nonsingular) {
                 const M3& T = e.T;
                 const float dL_da = cg.dL_da, dL_db = cg.dL_db, dL_dc = cg.dL_dc;
@@ -845,6 +895,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(con
         if (nrows > 0) warp_rows_out<3 * MT>(a.dL_dsh + (size_t)first * L, rows, L, nrows, lane);
     }
     if (!valid) return;
+    if (AA) a.dL_dopacity[idx] = aa_h * g[5];
     // like the reference, dL_dscale is taken w.r.t. (scale_modifier * scale) and is
     // not multiplied by the modifier (backward.cu:322-325)
     a.dL_dmean3D[3 * idx + 0] = dmean[0];

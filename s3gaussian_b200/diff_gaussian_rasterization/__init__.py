@@ -139,8 +139,20 @@ def _camera_inputs(raster_settings):
     return None
 
 
+def _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                       raster_settings, colors_aux, opacity):
+    """_RasterizeGaussians.apply of an antialiased forward: every optional input given, antialiasing last."""
+    cam = _camera_inputs(raster_settings)
+    return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                     cov3Ds_precomp, raster_settings, colors_aux,
+                                     *(cam if cam is not None else (None, None, None)), opacity, True)
+
+
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                        cov3Ds_precomp, raster_settings):
+                        cov3Ds_precomp, raster_settings, antialiasing=False):
+    if antialiasing:
+        return _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                  cov3Ds_precomp, raster_settings, None, False)
     cam = _camera_inputs(raster_settings)
     if cam is not None:
         return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales,
@@ -150,9 +162,12 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales,
 
 
 def rasterize_gaussians_aux(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                            cov3Ds_precomp, raster_settings, colors_aux):
+                            cov3Ds_precomp, raster_settings, colors_aux, antialiasing=False):
     """(color, radii, depth, color_aux): both colour sets composited on ONE preprocess + sort
     (the aux pair of s3g_rasterize_forward / s3g_rasterize_backward)."""
+    if antialiasing:
+        return _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                  cov3Ds_precomp, raster_settings, colors_aux, False)
     cam = _camera_inputs(raster_settings)
     if cam is not None:
         return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales,
@@ -162,9 +177,12 @@ def rasterize_gaussians_aux(means3D, means2D, sh, colors_precomp, opacities, sca
 
 
 def rasterize_gaussians_opacity(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                cov3Ds_precomp, raster_settings, colors_aux=None):
+                                cov3Ds_precomp, raster_settings, colors_aux=None, antialiasing=False):
     """(color, radii, depth, alpha, median_depth[, color_aux]): the opacity images of s3g_rasterize_forward_opacity
     from the same walk, differentiable like the others (the *_opacity backwards)."""
+    if antialiasing:
+        return _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                  cov3Ds_precomp, raster_settings, colors_aux, True)
     cam = _camera_inputs(raster_settings)
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                      cov3Ds_precomp, raster_settings, colors_aux,
@@ -214,7 +232,7 @@ def _forward_args(means3D, sh, colors_precomp, opacities, scales, rotations, cov
 
 
 def rasterize_gaussians_eval(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                             raster_settings, group=None, flow_colors=(), with_opacity=False):
+                             raster_settings, group=None, flow_colors=(), with_opacity=False, antialiasing=False):
     """s3g_rasterize_forward with its forward-only extras: (color, radii, depth, decomposition, flows) from one
     preprocess, one sort and one composite walk.  decomposition is (color_d, depth_d, color_s, depth_s) when
     `group` (bool or uint8 [P] on the device) is given, else None: the images forward() gives for the Gaussians
@@ -222,7 +240,8 @@ def rasterize_gaussians_eval(means3D, means2D, sh, colors_precomp, opacities, sc
     `flow_colors` (at most two float32 [P,4] device tensors, rgb in [:, :3], as s3g_flow_colors writes them), each
     the image forward() gives with colors_precomp = that rgb.  with_opacity adds a sixth element, (alpha,
     median_depth, alpha_d, alpha_s) as forward_opacity() defines them; alpha_d / alpha_s are the dynamic and static
-    subsets' alpha images, None without `group`.  Forward only: there is no autograd node."""
+    subsets' alpha images, None without `group`.  antialiasing: s3g_rasterize_forward_antialiased instead.  Forward
+    only: there is no autograd node."""
     lib = _lib.load()
     flow_colors = tuple(flow_colors)
     if len(flow_colors) > 2:
@@ -251,13 +270,17 @@ def rasterize_gaussians_eval(means3D, means2D, sh, colors_precomp, opacities, sc
         fwd.flow_colors[k], fwd.out_flow[k] = _ptr(fc), out.data_ptr()
     with torch.cuda.device(dev):
         if not with_opacity:
-            _lib.check(lib.s3g_rasterize_forward(C.byref(scene), C.byref(fwd), _stream_ptr(dev)),
-                       "rasterize_gaussians_eval")
+            if antialiasing:
+                _lib.check(lib.s3g_rasterize_forward_antialiased(C.byref(scene), C.byref(fwd), None,
+                                                                 _stream_ptr(dev)), "rasterize_gaussians_eval")
+            else:
+                _lib.check(lib.s3g_rasterize_forward(C.byref(scene), C.byref(fwd), _stream_ptr(dev)),
+                           "rasterize_gaussians_eval")
             return color, radii, depth, decomposition, flows
         opacity = tuple(torch.empty_like(depth) if i < 2 or group is not None else None for i in range(4))
         opa = _lib.RasterOpacityArgs(*(_ptr(t) for t in opacity))
-        _lib.check(lib.s3g_rasterize_forward_opacity(C.byref(scene), C.byref(fwd), C.byref(opa), _stream_ptr(dev)),
-                   "rasterize_gaussians_eval")
+        forward = lib.s3g_rasterize_forward_antialiased if antialiasing else lib.s3g_rasterize_forward_opacity
+        _lib.check(forward(C.byref(scene), C.byref(fwd), C.byref(opa), _stream_ptr(dev)), "rasterize_gaussians_eval")
     return color, radii, depth, decomposition, flows, opacity
 
 
@@ -316,10 +339,11 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                 cov3Ds_precomp, raster_settings, colors_aux=None, viewmatrix=None, projmatrix=None, campos=None,
-                opacity=False):
+                opacity=False, antialiasing=False):
         # viewmatrix / projmatrix / campos: raster_settings' own tensors, passed (by rasterize_gaussians*) only when
         # one of them requires grad; the backward then returns their gradients.  opacity (rasterize_gaussians_opacity):
-        # alpha and median_depth follow depth in the outputs
+        # alpha and median_depth follow depth in the outputs.  antialiasing: s3g_rasterize_forward_antialiased, whose
+        # chain rule the backward calls apply by themselves
         lib = _lib.load()
         rs = raster_settings
         scene, fwd, lease, inputs, color, depth, radii = _forward_args(means3D, sh, colors_precomp, opacities, scales,
@@ -336,6 +360,10 @@ class _RasterizeGaussians(torch.autograd.Function):
         if opacity:
             alpha, median_depth = torch.empty_like(depth), torch.empty_like(depth)
             opa = _lib.RasterOpacityArgs(out_alpha=alpha.data_ptr(), out_median_depth=median_depth.data_ptr())
+        if antialiasing:
+            forward_call = lambda: lib.s3g_rasterize_forward_antialiased(
+                C.byref(scene), C.byref(fwd), C.byref(opa) if opacity else None, _stream_ptr(dev))
+        elif opacity:
             forward_call = lambda: lib.s3g_rasterize_forward_opacity(C.byref(scene), C.byref(fwd), C.byref(opa),
                                                                      _stream_ptr(dev))
         else:
@@ -371,6 +399,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         if ctx.camera:
             ctx.cam_shapes = (rs.viewmatrix.shape, rs.projmatrix.shape, rs.campos.shape)
         ctx.opacity = bool(opacity)
+        ctx.antialiasing = bool(antialiasing)
         out = (color, radii, depth) + ((alpha, median_depth) if opacity else ()) + ((color_aux,) if has_aux else ())
         return out
 
@@ -378,6 +407,7 @@ class _RasterizeGaussians(torch.autograd.Function):
     def backward(ctx, grad_out_color, grad_radii, grad_depth, *grad_rest):
         # grad_rest: (grad_alpha, grad_median_depth) of an opacity forward, then grad_out_aux with the aux set
         opacity = getattr(ctx, "opacity", False)
+        antialiasing = getattr(ctx, "antialiasing", False)
         grad_alpha, grad_median = grad_rest[:2] if opacity else (None, None)
         grad_rest = grad_rest[2:] if opacity else grad_rest
         grad_out_aux = grad_rest[0] if grad_rest else None
@@ -447,6 +477,8 @@ class _RasterizeGaussians(torch.autograd.Function):
             # below are views of the exchange's bucket and hold the sums after its finish()
             if has_cov_in:
                 raise NotImplementedError("FusedGradExchange: precomputed 3-D covariances are not exchanged")
+            if antialiasing:
+                raise NotImplementedError("FusedGradExchange: an antialiased forward's gradients are not exchanged")
             _GRAD_SINK.note_backward()
             bwd.sink = C.pointer(peer)
         with torch.cuda.device(dev):
@@ -477,11 +509,13 @@ class _RasterizeGaussians(torch.autograd.Function):
         )
         if ctx.has_aux:
             grads = grads + (grad_aux,)
-        if ctx.camera or opacity:
+        if ctx.camera or opacity or antialiasing:
             if not ctx.has_aux:
                 grads = grads + (None,)
             grads = grads + (cam_grads if any(cam_needs) else (None, None, None))
-        if opacity:
+        if opacity or antialiasing:
+            grads = grads + (None,)
+        if antialiasing:
             grads = grads + (None,)
         return grads
 
@@ -515,9 +549,16 @@ def _reference_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp):
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings):
+    """antialiasing=True: every forward applies Mip-Splatting's 2-D screen-space filter (s3g_rasterize_forward_antialiased,
+    include/s3g_b200.h): each Gaussian's opacity is scaled by h = sqrt(max(det(cov2D) / det(cov2D + 0.3 I), 2.5e-5)),
+    so a Gaussian smaller than a pixel keeps its on-screen energy at every resolution.  The backwards, camera
+    gradients included, differentiate that forward.  Not in the reference (upstream 3DGS: `antialiasing`, gsplat:
+    rasterize_mode="antialiased")."""
+
+    def __init__(self, raster_settings, antialiasing=False):
         super().__init__()
         self.raster_settings = raster_settings
+        self.antialiasing = bool(antialiasing)
 
     def markVisible(self, positions):
         """bool[P]: passes the near-plane test (rasterizer_impl.cu:54-66)."""
@@ -541,7 +582,7 @@ class GaussianRasterizer(nn.Module):
         shs, colors_precomp, scales, rotations, cov3D_precomp = _reference_inputs(shs, colors_precomp, scales,
                                                                                   rotations, cov3D_precomp)
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales,
-                                   rotations, cov3D_precomp, self.raster_settings)
+                                   rotations, cov3D_precomp, self.raster_settings, self.antialiasing)
 
     def forward_aux(self, means3D, means2D, opacities, colors_aux, shs=None, colors_precomp=None, scales=None,
                     rotations=None, cov3D_precomp=None):
@@ -551,7 +592,7 @@ class GaussianRasterizer(nn.Module):
         shs, colors_precomp, scales, rotations, cov3D_precomp = _reference_inputs(shs, colors_precomp, scales,
                                                                                   rotations, cov3D_precomp)
         return rasterize_gaussians_aux(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                       cov3D_precomp, self.raster_settings, colors_aux)
+                                       cov3D_precomp, self.raster_settings, colors_aux, self.antialiasing)
 
     def forward_opacity(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                         cov3D_precomp=None, colors_aux=None):
@@ -564,7 +605,7 @@ class GaussianRasterizer(nn.Module):
         shs, colors_precomp, scales, rotations, cov3D_precomp = _reference_inputs(shs, colors_precomp, scales,
                                                                                   rotations, cov3D_precomp)
         return rasterize_gaussians_opacity(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                           cov3D_precomp, self.raster_settings, colors_aux)
+                                           cov3D_precomp, self.raster_settings, colors_aux, self.antialiasing)
 
     def forward_eval(self, means3D, means2D, opacities, group=None, flow_colors=(), shs=None, colors_precomp=None,
                      scales=None, rotations=None, cov3D_precomp=None, with_opacity=False):
@@ -581,4 +622,5 @@ class GaussianRasterizer(nn.Module):
         shs, colors_precomp, scales, rotations, cov3D_precomp = _reference_inputs(shs, colors_precomp, scales,
                                                                                   rotations, cov3D_precomp)
         return rasterize_gaussians_eval(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                        cov3D_precomp, self.raster_settings, group, flow_colors, with_opacity)
+                                        cov3D_precomp, self.raster_settings, group, flow_colors, with_opacity,
+                                        self.antialiasing)

@@ -166,7 +166,7 @@ def render_pixels(viewpoint_stack, gaussians, bg, pipe, compute_metrics: bool = 
     given; s3gaussian_b200.lpips.LPIPS() computes the reference's LPIPS on the device.  Not covered: save_seperate_pcd (render_func
     :243-249), which render_pixels never enables.
     """
-    from .gaussian_renderer import dynamic_mask_of, fine_front, raster_settings_for
+    from .gaussian_renderer import dynamic_mask_of, fine_front, pipe_rasterizer_kwargs, raster_settings_for
     from .diff_gaussian_rasterization import GaussianRasterizer
     rgbs, gt_rgbs, depths, static_rgbs, dynamic_rgbs = [], [], [], [], []
     opacities, median_depths, static_opacities, dynamic_opacities = [], [], [], []
@@ -204,7 +204,7 @@ def render_pixels(viewpoint_stack, gaussians, bg, pipe, compute_metrics: bool = 
                 if a not in colours:
                     colours[a] = flow_colors(dx_list[a + NUM_CAMS], dx_list[a], normalize=debug)
             group = dynamic_mask_of(dx) if return_decomposition and dx is not None else None
-            out = GaussianRasterizer(raster_settings=rs).forward_eval(
+            out = GaussianRasterizer(raster_settings=rs, **pipe_rasterizer_kwargs(pipe)).forward_eval(
                 means3D=means3D, means2D=torch.zeros_like(means3D), opacities=opacity, group=group,
                 flow_colors=[colours[a] for a in need], shs=shs, colors_precomp=colors_precomp, scales=scales,
                 rotations=rotations, **({"with_opacity": True} if with_opacity else {}))

@@ -75,6 +75,7 @@ class PipelineParams:       # arguments/__init__.py:93-98 defaults
     debug = False
     shared_binning = True   # ours: colour + feature image in one rasterizer pass (False = two passes, as upstream)
     render_opacity = False  # ours: render() also returns the alpha and median-depth images (and alpha_d / alpha_s)
+    antialiasing = False    # ours: the rasterizer's antialiasing filter (GaussianRasterizer(antialiasing=True))
 
 
 def pipe_shared_binning(pipe) -> bool:
@@ -83,6 +84,11 @@ def pipe_shared_binning(pipe) -> bool:
 
 def pipe_render_opacity(pipe) -> bool:
     return bool(getattr(pipe, "render_opacity", False))
+
+
+def pipe_rasterizer_kwargs(pipe) -> dict:
+    """The keyword arguments GaussianRasterizer takes from the pipeline parameters: none unless pipe.antialiasing."""
+    return {"antialiasing": True} if getattr(pipe, "antialiasing", False) else {}
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
@@ -99,7 +105,7 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
 
     raster_settings = raster_settings_for(viewpoint_camera, pc, pipe, bg_color, scaling_modifier)
     campos = raster_settings.campos
-    rasterizer = GaussianRasterizer(raster_settings=raster_settings)
+    rasterizer = GaussianRasterizer(raster_settings=raster_settings, **pipe_rasterizer_kwargs(pipe))
 
     means2D = screenspace_points
     shs = pc.get_features
