@@ -1,7 +1,7 @@
 """A minimal S3Gaussian-style training loop on the H100 path: the control flow of the reference's
 train.py (scene_reconstruction, train.py:330-530) with every heavy step running through libs3g_b200.so.
 
-    python examples/train_loop.py [--points 200000] [--iters 300] [--fine]
+    python examples/train_loop.py [--points 200000] [--iters 300] [--fine] [--filter-3d] [--densify-until N]
 
 Synthetic data (there is no dataset reader here): a random cloud initialised through create_from_pcd
 (3-NN scales), targets rendered from a perturbed copy of it.  Needs a CUDA device (sm_90a).
@@ -28,6 +28,9 @@ def main():
     ap.add_argument("--height", type=int, default=640)
     ap.add_argument("--fine", action="store_true", help="train the HexPlane deformation stage too")
     ap.add_argument("--checkpoint", default="", help="write and re-load a reference-format checkpoint here (needs --fine)")
+    ap.add_argument("--filter-3d", action="store_true",
+                    help="Mip-Splatting's 3-D smoothing filter, recomputed on Mip-Splatting's schedule")
+    ap.add_argument("--densify-until", type=int, default=0, help="last densification iteration (0: never stop)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("needs a CUDA device: s3gaussian_b200 has no CPU path")
@@ -36,6 +39,8 @@ def main():
     cams = [c.to(dev) for c in syn.waymo_ring(a.width, a.height, frames=10)]
     bg = torch.zeros(3, device=dev)
     pipe = PipelineParams()
+    train_pipe = PipelineParams()
+    train_pipe.filter_3d = a.filter_3d
 
     # ---- scene: "ground truth" cloud -> target images; training starts from a point cloud of it -------
     truth = syn.make_cloud(a.points, seed=0)
@@ -59,6 +64,8 @@ def main():
         deformation.deformation_net.set_aabb(*[list(x) for x in syn.WAYMO_AABB])
     gaussians = GaussianModel(3, deformation=deformation).create_from_pcd(pcd, spatial_lr_scale=5.0)   # 3-NN scales
     gaussians.training_setup(opt)
+    if a.filter_3d:
+        gaussians.compute_3D_filter(cams)       # Mip-Splatting: once before training, from every training camera
     stage = "fine" if a.fine else "coarse"
     extent = 30.0
 
@@ -70,7 +77,7 @@ def main():
         if it % 100 == 0:
             gaussians.oneupSHdegree()
         k = (it - 1) % len(cams)
-        out = render(cams[k], gaussians, pipe, bg, stage=stage, return_dx=a.fine, render_feat=False)
+        out = render(cams[k], gaussians, train_pipe, bg, stage=stage, return_dx=a.fine, render_feat=False)
         image, depth = out["render"], out["depth"]
         l1, ssim_value, depth_l2 = losses.image_loss_terms(image, targets[k][0], depth, targets[k][1])
         loss = l1 + 0.5 * depth_l2 + 0.2 * (1.0 - ssim_value)                    # train.py:395-419
@@ -80,10 +87,15 @@ def main():
         loss.backward()
         with torch.no_grad():
             gaussians.densification_step(out["viewspace_points"].grad, out["radii"])     # train.py:489-491
-            if it > 50 and it % 100 == 0:
+            densifying = not a.densify_until or it < a.densify_until
+            if densifying and it > 50 and it % 100 == 0:
                 gaussians.densify(0.0002, 0.005, extent, 20 if it > 3000 else None)
                 gaussians.prune(0.0002, 0.005, extent, 20 if it > 3000 else None)
                 gaussians.spatial_sort()      # ours: keep the model in Morton order (densify appends at the end)
+                if a.filter_3d:
+                    gaussians.compute_3D_filter(cams)     # Mip-Splatting: after every densify and prune
+            elif a.filter_3d and a.densify_until and it > a.densify_until and it % 100 == 0 and it < a.iters - 100:
+                gaussians.compute_3D_filter(cams)         # then every 100 iterations, except near the end
         gaussians.optimizer.step()                                               # one launch over all groups
         gaussians.optimizer.zero_grad(set_to_none=True)
         if it % 50 == 0:

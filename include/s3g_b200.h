@@ -286,6 +286,56 @@ int s3g_rasterize_backward_deterministic_opacity(const s3g_raster_scene* scene, 
 int64_t s3g_rasterize_forward_antialiased(const s3g_raster_scene* scene, const s3g_raster_forward_args* fwd,
                                           const s3g_raster_opacity_args* opa /* may be NULL */, void* stream);
 
+/* ---- 3-D smoothing filter (Mip-Splatting's compute_3D_filter, get_scaling / get_opacity_with_3D_filter) ----------
+ * Not in the reference.  Extends the model side of render(): optimisation lets a Gaussian shrink far below the finest
+ * sampling interval any training camera had at its position, and a view closer than every training camera (a lane
+ * change, a frame between two training frames) then shows it as a needle or speck.  The filter gives each Gaussian a
+ * world-space lower bound on its size from the training cameras' sampling rates; it is applied to the activated scales
+ * and opacities before the rasterizer (and its scale_modifier) and complements the 2-D antialiasing filter above, which
+ * handles the opposite case (a model rendered coarser than it was trained).
+ *
+ * s3g_filter3d_compute: xyz DEVICE float [P,3] the Gaussian means (in the fine stage the canonical, undeformed
+ * positions); C training cameras: viewmatrices DEVICE float [C,16], each the world-to-view matrix in the rasterizer's
+ * viewmatrix layout (m[k] = M[k%4][k/4]), cams DEVICE float [C,4] = (width, height, focal_x, focal_y) with
+ * focal_x = width / (2 tan(FoVx / 2)), focal_y likewise, all positive.  Writes filter_3d DEVICE float [P]:
+ *   1. for camera c and Gaussian i, (x, y, z) the camera-space mean, u = x / z focal_x + width / 2,
+ *      v = y / z focal_y + height / 2;
+ *   2. the pair is valid when z > 0.2, -0.15 width <= u <= 1.15 width and -0.15 height <= v <= 1.15 height (taken in
+ *      the multiplied form |x focal_x| <= 0.65 width z, the camera-space mean in double);
+ *   3. d_i = min over the valid cameras of z;
+ *   4. F = max over ALL cameras of focal_x - Mip-Splatting's choice: one focal for the whole camera set, not the min
+ *      of z / focal per camera;
+ *   5. a Gaussian no camera sees gets d_i = the max of d over the Gaussians that have one; when no Gaussian is seen,
+ *      every filter value is 0 (Mip-Splatting raises there);
+ *   6. filter_3d[i] = d_i / F * sqrt(0.2), 0.2 px^2 being Mip-Splatting's fixed variance.
+ * Only min and max are taken, so two calls give bitwise equal results.  Three launches (a 4-byte memset, the depth
+ * pass with the cameras staged through shared memory 64 at a time, the fill pass); no host synchronisation.
+ * workspace: s3g_filter3d_compute_workspace_bytes(P) bytes (16 for P > 0, 0 otherwise), 16-byte aligned.  P == 0
+ * does nothing and returns S3G_OK.
+ * S3G_ERR_ARG before any launch: P < 0; C < 1 with P > 0; a NULL pointer; an unaligned workspace; P > INT_MAX / 3 or
+ * C > INT_MAX / 16 (32-bit element indices).
+ *
+ * s3g_filter3d_apply_forward: scales DEVICE float [P,3] (activated, > 0), opacity [P] (activated), filter_3d [P] ->
+ *   out_scales[i,k]  = sqrt(scales[i,k]^2 + f^2),
+ *   out_opacity[i]   = opacity[i] sqrt(prod_k scales[i,k]^2 / prod_k out_scales[i,k]^2)   (f = filter_3d[i]),
+ * which keeps opacity * prod scales, the Gaussian's integrated density.  Where f = 0 (and scales^2 is a normal
+ * float) the outputs equal the inputs bitwise.
+ * s3g_filter3d_apply_backward: the same inputs and the upstream gradients g_out_scales [P,3], g_out_opacity [P] ->
+ *   g_scales[i,k] = g_out_scales[i,k] s_k / s'_k + g_out_opacity[i] o' f^2 / (s_k s'_k^2),
+ *   g_opacity[i]  = g_out_opacity[i] sqrt(prod_k s_k^2 / prod_k s'_k^2)
+ * (s = scales, s' = out_scales, o' = out_opacity); the filter is a constant and gets no gradient.  Where f = 0 the
+ * gradients pass through bitwise.
+ * One launch each; every output is written in full and must not alias an input.  P == 0 does nothing.
+ * S3G_ERR_ARG before any launch: P < 0, a NULL pointer, P > INT_MAX / 3. */
+size_t s3g_filter3d_compute_workspace_bytes(int P);
+int s3g_filter3d_compute(int P, const float* xyz, int C, const float* viewmatrices, const float* cams,
+                         float* filter_3d, void* workspace, void* stream);
+int s3g_filter3d_apply_forward(int P, const float* scales, const float* opacity, const float* filter_3d,
+                               float* out_scales, float* out_opacity, void* stream);
+int s3g_filter3d_apply_backward(int P, const float* scales, const float* opacity, const float* filter_3d,
+                                const float* g_out_scales, const float* g_out_opacity, float* g_scales,
+                                float* g_opacity, void* stream);
+
 /* ---- camera gradients ---------------------------------------------------------------------------------------------
  * Extends the backward of _RasterizeGaussians (DGR/diff_gaussian_rasterization/__init__.py:101-156), which returns no
  * gradient for raster_settings, and Rasterizer::backward (rasterizer.h:58-88): the gradient of the same loss with

@@ -36,6 +36,10 @@ SIGNATURES = {
     "s3g_rasterize_backward_deterministic_opacity": (_I, [_V, _V, _V, _V, _V]),
     # s3g_rasterize_forward_opacity with the antialiasing filter; the RasterOpacityArgs may be NULL
     "s3g_rasterize_forward_antialiased": (_I64, [_V, _V, _V, _V]),
+    "s3g_filter3d_compute_workspace_bytes": (_SZ, [_I]),
+    "s3g_filter3d_compute": (_I, [_I, _V, _I, _V, _V, _V, _V, _V]),
+    "s3g_filter3d_apply_forward": (_I, [_I, _V, _V, _V, _V, _V, _V]),
+    "s3g_filter3d_apply_backward": (_I, [_I, _V, _V, _V, _V, _V, _V, _V, _V]),
     # s3g_rasterize_camera_backward also takes a RasterCameraGrads (below) with ctypes.byref()
     "s3g_rasterize_camera_backward_workspace_bytes": (_SZ, [_I]),
     "s3g_rasterize_camera_backward": (_I, [_V, _V, _V, _V, _V]),

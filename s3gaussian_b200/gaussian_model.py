@@ -21,6 +21,12 @@ match the reference bit for bit (tests/test_gpu_train.py runs the reference's ow
 
 ``create_from_pcd`` uses our distCUDA2 (simple_knn.py, csrc/knn.cuh); ``save_ply`` / ``load_ply`` keep the
 reference's attribute layout (io_ply.py).  CUDA only; no CPU path.
+
+Not in the reference: Mip-Splatting's 3-D smoothing filter (filter3d.py).  ``compute_3D_filter(cameras)`` fills
+``filter_3D`` [P,1]; ``get_scaling_with_3D_filter`` / ``get_opacity_with_3D_filter`` apply it, and render() does with
+``pipe.filter_3d``.  Densify, prune and ``spatial_sort`` carry it (a new row takes its source row's value) until the
+loop recomputes it.  It is not saved: ``capture()`` / ``restore()`` and the .ply files keep the reference's layout, so
+recompute it from the training cameras after loading.
 """
 from __future__ import annotations
 
@@ -90,6 +96,7 @@ class GaussianModel:
         self._xyz = self._features_dc = self._features_rest = self._scaling = self._rotation = self._opacity = e
         self.max_radii2D = self.xyz_gradient_accum = self.denom = self._deformation_accum = e
         self._deformation_table = e
+        self.filter_3D = e              # [P,1] once compute_3D_filter() ran; empty until then
         self.optimizer = None
         self.percent_dense = 0
         self.spatial_lr_scale = 0
@@ -115,6 +122,7 @@ class GaussianModel:
         P = xyz.shape[0]
         self.max_radii2D = torch.zeros(P, device=dev)
         self._deformation_table = torch.ones(P, dtype=torch.bool, device=dev)
+        self.filter_3D = torch.empty(0, device=dev)
         return self
 
     def create_from_pcd(self, pcd, spatial_lr_scale: float):
@@ -195,6 +203,31 @@ class GaussianModel:
     def get_opacity(self):
         return self.opacity_activation(self._opacity)
 
+    # ---- Mip-Splatting's 3-D smoothing filter (filter3d.py) -------------------------------------------------------
+    def compute_3D_filter(self, cameras):
+        """filter_3D <- the filter of the current (canonical) positions from the training cameras."""
+        from .filter3d import compute_filter_3d
+        self.filter_3D = compute_filter_3d(self.get_xyz, cameras)
+
+    def _require_filter_3D(self):
+        if self.filter_3D.dim() != 2 or self.filter_3D.shape[0] != self._xyz.shape[0]:
+            raise RuntimeError(f"filter_3D has {tuple(self.filter_3D.shape)} rows for {self._xyz.shape[0]} Gaussians: "
+                               "call compute_3D_filter(cameras) first")
+
+    # Each of the two properties runs the apply kernel and keeps half of its result, as Mip-Splatting's pair does; to
+    # read both in one launch, call filter3d.apply_filter_3d(self.get_scaling, self.get_opacity, self.filter_3D).
+    @property
+    def get_scaling_with_3D_filter(self):
+        from .filter3d import apply_filter_3d
+        self._require_filter_3D()
+        return apply_filter_3d(self.get_scaling, self.get_opacity, self.filter_3D)[0]
+
+    @property
+    def get_opacity_with_3D_filter(self):
+        from .filter3d import apply_filter_3d
+        self._require_filter_3D()
+        return apply_filter_3d(self.get_scaling, self.get_opacity, self.filter_3D)[1]
+
     def get_covariance(self, scaling_modifier=1):
         from .gaussian_renderer import GaussianModelLite
         return GaussianModelLite.get_covariance(self, scaling_modifier)
@@ -271,6 +304,7 @@ class GaussianModel:
         self._xyz, self._features_dc, self._features_rest = mk(xyz), mk(f_dc), mk(f_rest)
         self._scaling, self._rotation, self._opacity = mk(scaling), mk(rotation), mk(opacity)
         self._deformation_table = table.to(dev)
+        self.filter_3D = torch.empty(0, device=dev)     # not in the tuple: recompute it from the cameras
         self.max_radii2D = max_radii2D.to(dev)
         self._deformation = self._deformation.to(dev)
         self._deformation.load_state_dict(deform_state)
@@ -322,6 +356,9 @@ class GaussianModel:
                 new_states[name] = (st["step"], add(st["exp_avg"], True), add(st["exp_avg_sq"], True))
         acc = None
         P_old = self._xyz.shape[0]
+        # the 3-D filter, while it matches the rows: new rows take their source row's value
+        filt = (add(self.filter_3D.to(dev, torch.float32), False)
+                if self.filter_3D.dim() == 2 and self.filter_3D.shape[0] == P_old else None)
         have_acc = all(t.numel() > 0 and t.shape[0] == P_old for t in
                        (self.xyz_gradient_accum, self.denom, self._deformation_accum, self.max_radii2D))
         if keep_accumulators and not have_acc:      # training_setup() not called yet: nothing to carry over
@@ -345,6 +382,7 @@ class GaussianModel:
                     self.optimizer.state[newp] = {"step": step, "exp_avg": m, "exp_avg_sq": v}
             setattr(self, _ATTR[name], newp)
         self._deformation_table = self._deformation_table[src_index]
+        self.filter_3D = filt if filt is not None else torch.empty(0, device=dev)
         if keep_accumulators:
             self.xyz_gradient_accum, self.denom, self._deformation_accum = acc[0], acc[1], acc[2]
             self.max_radii2D = acc[3].squeeze(1)

@@ -19,6 +19,7 @@ import torch
 import torch.nn as nn
 
 from .diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer
+from .filter3d import apply_filter_3d
 
 
 class GaussianModelLite(nn.Module):
@@ -76,6 +77,7 @@ class PipelineParams:       # arguments/__init__.py:93-98 defaults
     shared_binning = True   # ours: colour + feature image in one rasterizer pass (False = two passes, as upstream)
     render_opacity = False  # ours: render() also returns the alpha and median-depth images (and alpha_d / alpha_s)
     antialiasing = False    # ours: the rasterizer's antialiasing filter (GaussianRasterizer(antialiasing=True))
+    filter_3d = False       # ours: Mip-Splatting's 3-D smoothing filter on the scales and opacities (pc.filter_3D)
 
 
 def pipe_shared_binning(pipe) -> bool:
@@ -91,9 +93,26 @@ def pipe_rasterizer_kwargs(pipe) -> dict:
     return {"antialiasing": True} if getattr(pipe, "antialiasing", False) else {}
 
 
+def pipe_filter_3d(pipe, pc) -> bool:
+    """Whether pipe.filter_3d is set; when it is, checks before any launch that `pc` has a filter_3D for its P
+    Gaussians and that precomputed covariances are not asked for."""
+    if not getattr(pipe, "filter_3d", False):
+        return False
+    if pipe.compute_cov3D_python:
+        raise NotImplementedError("pipe.filter_3d with compute_cov3D_python: the 3-D filter applies to scales, not "
+                                  "precomputed covariances")
+    P = pc.get_xyz.shape[0]
+    f = getattr(pc, "filter_3D", None)
+    if f is None or f.dim() != 2 or f.shape[0] != P:
+        raise RuntimeError(f"pipe.filter_3d: the model has no filter_3D for its {P} Gaussians "
+                           f"({None if f is None else tuple(f.shape)}); call compute_3D_filter(cameras) first")
+    return True
+
+
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
            stage="fine", return_decomposition=False, return_dx=False, render_feat=False):
     """Render the scene.  Background tensor (bg_color) must be on GPU!"""
+    filter_3d = pipe_filter_3d(pipe, pc)
     xyz = pc.get_xyz
     dev = xyz.device
     # gradient carrier for the 2-D means (gaussian_renderer/__init__.py:31-35)
@@ -121,6 +140,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
             scales_final = pc.scaling_activation(pc._scaling)
             rotations_final = pc.rotation_activation(pc._rotation)
         opacity = pc.opacity_activation(pc._opacity)
+        if filter_3d:
+            scales_final, opacity = apply_filter_3d(scales_final, opacity, pc.filter_3D)
         shs_final, colors_precomp = shs, None
         # convert_SHs_python evaluates the same polynomial with dir = xyz - campos; in the coarse
         # stage the rasterized mean IS xyz, so the in-kernel SH path gives the same colours
@@ -233,7 +254,8 @@ def fine_front(viewpoint_camera, pc, pipe, campos, shs):
     """The fine stage's front end of render() (gaussian_renderer/__init__.py:85-117): deformation at the camera's time,
     activations and the colours or SHs the rasterizer takes; `shs` is pc.get_features.  One deformation forward.
     -> (means3D, scales, rotations, opacity, shs, colors_precomp, dx, dshs, feat); exactly one of shs /
-    colors_precomp is None."""
+    colors_precomp is None.  With pipe.filter_3d the scales and opacities are those after pc.filter_3D."""
+    filter_3d = pipe_filter_3d(pipe, pc)
     if pipe.compute_cov3D_python:
         raise NotImplementedError("compute_cov3D_python with the deformation stage (reference default: False)")
     xyz = pc.get_xyz
@@ -259,6 +281,8 @@ def fine_front(viewpoint_camera, pc, pipe, campos, shs):
         if pipe.convert_SHs_python:
             colors_precomp = _sh_python(pc, shs_final, xyz, campos)
             shs_final = None
+    if filter_3d:
+        scales_final, opacity = apply_filter_3d(scales_final, opacity, pc.filter_3D)
     return means3D_final, scales_final, rotations_final, opacity, shs_final, colors_precomp, dx, dshs, feat
 
 
