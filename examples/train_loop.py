@@ -2,6 +2,7 @@
 train.py (scene_reconstruction, train.py:330-530) with every heavy step running through libs3g_b200.so.
 
     python examples/train_loop.py [--points 200000] [--iters 300] [--fine] [--filter-3d] [--densify-until N]
+                                 [--absgrad-threshold T]
 
 Synthetic data (there is no dataset reader here): a random cloud initialised through create_from_pcd
 (3-NN scales), targets rendered from a perturbed copy of it.  Needs a CUDA device (sm_90a).
@@ -31,6 +32,9 @@ def main():
     ap.add_argument("--filter-3d", action="store_true",
                     help="Mip-Splatting's 3-D smoothing filter, recomputed on Mip-Splatting's schedule")
     ap.add_argument("--densify-until", type=int, default=0, help="last densification iteration (0: never stop)")
+    ap.add_argument("--absgrad-threshold", type=float, default=0.0,
+                    help="densify on the absolute screen-space gradient (AbsGS, gsplat absgrad) with this threshold "
+                         "instead of the signed one (0: off)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("needs a CUDA device: s3gaussian_b200 has no CPU path")
@@ -41,6 +45,7 @@ def main():
     pipe = PipelineParams()
     train_pipe = PipelineParams()
     train_pipe.filter_3d = a.filter_3d
+    train_pipe.absgrad = a.absgrad_threshold > 0
 
     # ---- scene: "ground truth" cloud -> target images; training starts from a point cloud of it -------
     truth = syn.make_cloud(a.points, seed=0)
@@ -86,10 +91,12 @@ def main():
                 gaussians.compute_regulation(0.01, 0.0001, 0.0001)
         loss.backward()
         with torch.no_grad():
-            gaussians.densification_step(out["viewspace_points"].grad, out["radii"])     # train.py:489-491
+            vs = out["viewspace_points"]
+            gaussians.densification_step(vs.grad, out["radii"], getattr(vs, "absgrad", None))   # train.py:489-491
             densifying = not a.densify_until or it < a.densify_until
             if densifying and it > 50 and it % 100 == 0:
-                gaussians.densify(0.0002, 0.005, extent, 20 if it > 3000 else None)
+                gaussians.densify(0.0002, 0.005, extent, 20 if it > 3000 else None,
+                                  max_grad_abs=a.absgrad_threshold if a.absgrad_threshold > 0 else None)
                 gaussians.prune(0.0002, 0.005, extent, 20 if it > 3000 else None)
                 gaussians.spatial_sort()      # ours: keep the model in Morton order (densify appends at the end)
                 if a.filter_3d:

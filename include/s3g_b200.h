@@ -286,6 +286,37 @@ int s3g_rasterize_backward_deterministic_opacity(const s3g_raster_scene* scene, 
 int64_t s3g_rasterize_forward_antialiased(const s3g_raster_scene* scene, const s3g_raster_forward_args* fwd,
                                           const s3g_raster_opacity_args* opa /* may be NULL */, void* stream);
 
+/* ---- absolute screen-space gradients (AbsGS; gsplat rasterization(absgrad=True), means2d.absgrad) ------------------
+ * Not in the reference.  Densification selects on the norm of the signed dL/dmean2D summed over pixels; over a large
+ * Gaussian on a textured surface the pixels pull in opposite directions, the sum cancels and the Gaussian is never
+ * split.  The absolute statistic sums each pixel's contribution's magnitude instead.  For Gaussian i, in the units of
+ * dL_dmean2D (the pixel offset times width/2 or height/2):
+ *   dL_dmean2D_abs[i] = ( sum_p |dL_p/dmean2D_x[i]|, sum_p |dL_p/dmean2D_y[i]| )
+ * over the pixels p it contributes to, where dL_p/dmean2D is pixel p's whole share of dL_dmean2D: every image of the
+ * call (colour, depth, the aux image, alpha and median depth) and the background term.  With X_p = G dL/dalpha_p,
+ * d_p = mean2D - pixel, (A, B, C) the conic and o the opacity the composite used (opacity * h after an antialiased
+ * forward):
+ *   x: o (width/2)  sum_p |X_p (A dx_p + B dy_p)|        y: o (height/2) sum_p |X_p (C dy_p + B dx_p)|
+ * The signed dL_dmean2D is the same sum without the absolute values, so |dL_dmean2D| <= dL_dmean2D_abs componentwise.
+ * The statistic belongs to one call: with the aux pair, each pixel's colour and aux terms are added before the absolute
+ * value; two separate calls for the two images add two sums of absolute values, which is never less.
+ *
+ * s3g_rasterize_backward_absgrad is s3g_rasterize_backward_opacity (`opa` may be NULL: s3g_rasterize_backward) or,
+ * with deterministic != 0, s3g_rasterize_backward_deterministic_opacity with `workspace` as there: the same scene,
+ * arguments, contract and every other output, the chain rule of an antialiased forward included.  It also writes
+ * dL_dmean2D_abs DEVICE float [P,2], zero where radii <= 0.  The composite keeps the two sums in entries 13 and 14 of
+ * each Gaussian's gradient record, which the other walks leave unused, so the geometry buffer and the workspace sizes
+ * are unchanged.  The deterministic form stays bitwise repeatable, dL_dmean2D_abs included; the default form adds
+ * with unordered atomics and differs in the last bits from call to call.  With a peer sink (deterministic = 0),
+ * dL_dmean2D_abs stays local like dL_dmean2D.
+ * S3G_ERR_ARG before any launch: every case of the call it extends; a NULL dL_dmean2D_abs when P > 0; deterministic
+ * with a peer sink. */
+int s3g_rasterize_backward_absgrad(const s3g_raster_scene* scene, const s3g_raster_backward_args* bwd,
+                                   const s3g_raster_opacity_args* opa /* may be NULL */,
+                                   float* dL_dmean2D_abs /* DEVICE [P,2] */, int deterministic,
+                                   void* workspace /* deterministic: as s3g_rasterize_backward_deterministic */,
+                                   void* stream);
+
 /* ---- 3-D smoothing filter (Mip-Splatting's compute_3D_filter, get_scaling / get_opacity_with_3D_filter) ----------
  * Not in the reference.  Extends the model side of render(): optimisation lets a Gaussian shrink far below the finest
  * sampling interval any training camera had at its position, and a view closer than every training camera (a lane
@@ -636,6 +667,12 @@ int s3g_adam_step(int n, const s3g_adam_tensor* tensors, double beta1, double be
  * for radii > 0: max_radii2D = max(max_radii2D, radii); xyz_gradient_accum += |grad[:2]|; denom += 1. */
 int s3g_densify_stats(int P, const float* viewspace_grad, const int* radii, float* xyz_gradient_accum,
                       float* denom, float* max_radii2D, void* stream);
+
+/* s3g_densify_stats in the same launch, and for radii > 0 also xyz_gradient_accum_abs += |viewspace_absgrad|, the
+ * L2 norm of the absolute screen-space gradient f32[P,2] (s3g_rasterize_backward_absgrad, summed over the views). */
+int s3g_densify_stats_abs(int P, const float* viewspace_grad, const float* viewspace_absgrad, const int* radii,
+                          float* xyz_gradient_accum, float* xyz_gradient_accum_abs, float* denom, float* max_radii2D,
+                          void* stream);
 
 /* image, gt_image: f32[B,C,H,W] (or C == 0 and NULL: depth term only); depth, gt_depth: f32[B,H,W] or
  * both NULL (no depth term).

@@ -36,6 +36,9 @@ SIGNATURES = {
     "s3g_rasterize_backward_deterministic_opacity": (_I, [_V, _V, _V, _V, _V]),
     # s3g_rasterize_forward_opacity with the antialiasing filter; the RasterOpacityArgs may be NULL
     "s3g_rasterize_forward_antialiased": (_I64, [_V, _V, _V, _V]),
+    # the backward with the absolute screen-space gradients: RasterOpacityArgs or NULL, dL_dmean2D_abs, deterministic,
+    # workspace
+    "s3g_rasterize_backward_absgrad": (_I, [_V, _V, _V, _V, _I, _V, _V]),
     "s3g_filter3d_compute_workspace_bytes": (_SZ, [_I]),
     "s3g_filter3d_compute": (_I, [_I, _V, _I, _V, _V, _V, _V, _V]),
     "s3g_filter3d_apply_forward": (_I, [_I, _V, _V, _V, _V, _V, _V]),
@@ -82,6 +85,7 @@ SIGNATURES = {
     # training-step kernels; s3g_adam_step takes a host array of AdamTensor (below)
     "s3g_adam_step": (_I, [_I, _V, _D, _D, _D, _V]),
     "s3g_densify_stats": (_I, [_I, _V, _V, _V, _V, _V, _V]),
+    "s3g_densify_stats_abs": (_I, [_I, _V, _V, _V, _V, _V, _V, _V, _V]),
     "s3g_image_loss_workspace_bytes": (_SZ, [_I, _I, _I, _I]),
     "s3g_image_loss_forward": (_I, [_I, _I, _I, _I, _V, _V, _V, _V, _F, _V, _V, _V]),
     "s3g_image_l1_depth_forward": (_I, [_I, _I, _I, _I, _V, _V, _V, _V, _F, _V, _V, _V]),

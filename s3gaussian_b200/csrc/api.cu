@@ -577,39 +577,47 @@ int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f
 
 // one backward composite walk (the default walk takes the RenderBwdArgs part of ra); > 48 KB of dynamic shared memory
 // needs the opt-in, once per (kernel, device)
-template <bool AUX, bool DET, bool OPA>
+template <bool AUX, bool DET, bool OPA, bool ABS>
 int launch_render_backward(const RenderBwdDetArgs& ra, const TileGrid& tg, cudaStream_t stream) {
     static unsigned long long attr_done = 0;
     int devid = 0;
     S3G_CUDA(cudaGetDevice(&devid), "cudaGetDevice");
     if (devid >= 64 || !((attr_done >> devid) & 1ull)) {
-        S3G_CUDA(cudaFuncSetAttribute(render_backward_kernel<AUX, DET, OPA>,
+        S3G_CUDA(cudaFuncSetAttribute(render_backward_kernel<AUX, DET, OPA, ABS>,
                                       cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)sizeof(RenderBwdSmem<AUX, DET, OPA>)),
+                                      (int)sizeof(RenderBwdSmem<AUX, DET, OPA, ABS>)),
                  DET ? "render_backward_det smem attribute" : "render_backward smem attribute");
         if (devid < 64) attr_done |= 1ull << devid;
     }
-    render_backward_kernel<AUX, DET, OPA>
-        <<<dim3(tg.x, tg.y), TILE_PIX, sizeof(RenderBwdSmem<AUX, DET, OPA>), stream>>>(ra);
+    render_backward_kernel<AUX, DET, OPA, ABS>
+        <<<dim3(tg.x, tg.y), TILE_PIX, sizeof(RenderBwdSmem<AUX, DET, OPA, ABS>), stream>>>(ra);
     return S3G_OK;
 }
-template <bool DET>
+template <bool DET, bool ABS>
 int launch_render_backward(bool aux, bool opa, const RenderBwdDetArgs& ra, const TileGrid& tg, cudaStream_t stream) {
-    if (opa) return aux ? launch_render_backward<true, DET, true>(ra, tg, stream)
-                        : launch_render_backward<false, DET, true>(ra, tg, stream);
-    return aux ? launch_render_backward<true, DET, false>(ra, tg, stream)
-               : launch_render_backward<false, DET, false>(ra, tg, stream);
+    if (opa) return aux ? launch_render_backward<true, DET, true, ABS>(ra, tg, stream)
+                        : launch_render_backward<false, DET, true, ABS>(ra, tg, stream);
+    return aux ? launch_render_backward<true, DET, false, ABS>(ra, tg, stream)
+               : launch_render_backward<false, DET, false, ABS>(ra, tg, stream);
+}
+template <bool DET>
+int launch_render_backward(bool aux, bool opa, bool abs, const RenderBwdDetArgs& ra, const TileGrid& tg,
+                           cudaStream_t stream) {
+    return abs ? launch_render_backward<DET, true>(aux, opa, ra, tg, stream)
+               : launch_render_backward<DET, false>(aux, opa, ra, tg, stream);
 }
 
 // det: the deterministic destination of the backward composite walk (composite.cuh) with det_ws as its workspace,
 // instead of the REDs into grad_rec; everything else, validation included, is shared.
-// o: the opacity-image gradients (the *_opacity entry points), or NULL
+// o: the opacity-image gradients (the *_opacity entry points), or NULL.
+// absgrad: the absolute screen-space gradients as well (s3g_rasterize_backward_absgrad), written to dL_dmean2D_abs
 int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, const s3g_raster_opacity_args* o,
-                  cudaStream_t stream, bool det, void* det_ws) {
+                  cudaStream_t stream, bool det, void* det_ws, bool absgrad = false, float* dL_dmean2D_abs = nullptr) {
     const int P = s.P, width = s.width, height = s.height, debug = s.debug;
     const s3g_peer_sink* sink = b.sink;
     if (P < 0 || width <= 0 || height <= 0 || b.R < 0) return fail(S3G_ERR_ARG, "backward: bad sizes");
     if (P == 0) return S3G_OK;   // rasterize_points.cu:165
+    if (absgrad && !dL_dmean2D_abs) return fail(S3G_ERR_ARG, "backward_absgrad: null dL_dmean2D_abs");
     if (!b.geom_buffer || !b.image_buffer || (b.R > 0 && !b.binning_buffer))
         return fail(S3G_ERR_STATE, "backward: missing state buffer");
     if (!s.means3D || !s.viewmatrix || !s.projmatrix || !s.background || !b.dL_dpix || !b.dL_dpix_depth)
@@ -679,12 +687,12 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
         det_base_kernel<<<(P + 255) / 256, 256, 0, stream>>>((uint32_t)P, geom.order_a, geom.offsets, base);
         S3G_STAGE("det_base");
         S3G_MARK(1, "render_backward_det");
-        const int rc = launch_render_backward<true>(use_aux, use_opa, ra, tg, stream);
+        const int rc = launch_render_backward<true>(use_aux, use_opa, absgrad, ra, tg, stream);
         if (rc != S3G_OK) return rc;
         S3G_STAGE("render_backward_det");
         S3G_MARK(1, "grad_rec_gather");
         grad_rec_gather_kernel<<<(unsigned)div_up64((int64_t)P * 4, 256), 256, 0, stream>>>(
-            (uint32_t)P, use_aux ? 4 : 3, geom.tiles_touched, base, records, reinterpret_cast<float4*>(geom.grad_rec));
+            (uint32_t)P, (use_aux || absgrad) ? 4 : 3, geom.tiles_touched, base, records, reinterpret_cast<float4*>(geom.grad_rec));
         S3G_STAGE("grad_rec_gather");
     } else {
         S3G_MARK(1, "zero_grad_rec");
@@ -692,7 +700,7 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
                  "memset grad_rec");
         S3G_MARK(1, "render_backward");
         if (b.R > 0) {
-            const int rc = launch_render_backward<false>(use_aux, use_opa, ra, tg, stream);
+            const int rc = launch_render_backward<false>(use_aux, use_opa, absgrad, ra, tg, stream);
             if (rc != S3G_OK) return rc;
             S3G_STAGE("render_backward");
         }
@@ -735,6 +743,12 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
         if (rc != S3G_OK) return rc;
     }
     S3G_STAGE("preprocess_backward");
+    if (absgrad) {
+        S3G_MARK(1, "absgrad_export");
+        absgrad_export_kernel<<<(P + 255) / 256, 256, 0, stream>>>((uint32_t)P, radii, geom.grad_rec,
+                                                                   dL_dmean2D_abs);
+        S3G_STAGE("absgrad_export");
+    }
     S3G_MARK(1, nullptr);
     return S3G_OK;
 }
@@ -785,6 +799,14 @@ int s3g_rasterize_backward_deterministic_opacity(const s3g_raster_scene* scene, 
                                                  const s3g_raster_opacity_args* opa, void* workspace, void* stream) {
     if (!scene || !bwd) return fail(S3G_ERR_ARG, "backward_deterministic_opacity: null scene / backward arguments");
     return backward_impl(*scene, *bwd, opa, static_cast<cudaStream_t>(stream), true, workspace);
+}
+
+int s3g_rasterize_backward_absgrad(const s3g_raster_scene* scene, const s3g_raster_backward_args* bwd,
+                                   const s3g_raster_opacity_args* opa, float* dL_dmean2D_abs, int deterministic,
+                                   void* workspace, void* stream) {
+    if (!scene || !bwd) return fail(S3G_ERR_ARG, "backward_absgrad: null scene / backward arguments");
+    return backward_impl(*scene, *bwd, opa, static_cast<cudaStream_t>(stream), deterministic != 0, workspace, true,
+                         dL_dmean2D_abs);
 }
 
 size_t s3g_rasterize_camera_backward_workspace_bytes(int P) {

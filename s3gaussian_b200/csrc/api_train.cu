@@ -67,6 +67,22 @@ int s3g_densify_stats(int P, const float* viewspace_grad, const int* radii, floa
     return S3G_OK;
 }
 
+int s3g_densify_stats_abs(int P, const float* viewspace_grad, const float* viewspace_absgrad, const int* radii,
+                          float* xyz_gradient_accum, float* xyz_gradient_accum_abs, float* denom, float* max_radii2D,
+                          void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (P < 0) return fail(S3G_ERR_ARG, "densify_stats_abs: P < 0");
+    if (P == 0) return S3G_OK;
+    if (!viewspace_grad || !viewspace_absgrad || !radii || !xyz_gradient_accum || !xyz_gradient_accum_abs || !denom ||
+        !max_radii2D)
+        return fail(S3G_ERR_ARG, "densify_stats_abs: null pointer");
+    densify_stats_abs_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, viewspace_grad, viewspace_absgrad, radii,
+                                                                  xyz_gradient_accum, xyz_gradient_accum_abs, denom,
+                                                                  max_radii2D);
+    S3G_CUDA(cudaGetLastError(), "densify_stats_abs launch");
+    return S3G_OK;
+}
+
 namespace {
 constexpr int kDepthBlocks = 592;    // 4 per SM
 struct LossPlan {

@@ -465,48 +465,74 @@ struct BwdMedianSlots {
 };
 template <>
 struct BwdMedianSlots<false> {};
-template <bool AUX, bool DET, bool OPA>
+// ABS: the walk also keeps the absolute screen-space gradients in record entries 13 and 14, so quarter 3 is written
+// with or without AUX
+template <bool AUX, bool DET, bool OPA, bool ABS = false>
 struct RenderBwdSmem : BwdWalkSmem<AUX, BCB>, BwdMedianSlots<OPA> {
     uint32_t max_contrib;
 };
-template <bool AUX, bool OPA>
-struct RenderBwdSmem<AUX, true, OPA> : BwdWalkSmem<AUX, DCB>, BwdMedianSlots<OPA> {
-    float4 part[AUX ? 4 : 3][8][DCB];      // [record quarter][warp][batch slot]; zero unless written this batch
+template <bool AUX, bool OPA, bool ABS>
+struct RenderBwdSmem<AUX, true, OPA, ABS> : BwdWalkSmem<AUX, DCB>, BwdMedianSlots<OPA> {
+    float4 part[(AUX || ABS) ? 4 : 3][8][DCB];   // [record quarter][warp][batch slot]; zero unless written this batch
     uint32_t max_contrib;
 };
 
 // quarter q of a flushed record to its destination: row g of grad_rec, or this warp's partial of batch slot `slot`
 // (DET).  Each batch slot is flushed at most once per warp and batch.
-template <bool AUX, bool DET, bool OPA>
-__device__ __forceinline__ void bwd_store(RenderBwdSmem<AUX, DET, OPA>& sm, int warp, float* g, int slot, int q, float4 v) {
+template <bool AUX, bool DET, bool OPA, bool ABS = false>
+__device__ __forceinline__ void bwd_store(RenderBwdSmem<AUX, DET, OPA, ABS>& sm, int warp, float* g, int slot, int q,
+                                          float4 v) {
     if constexpr (DET) {
         sm.part[q][warp][slot] = v;
     } else {
-        if (q == 3) atomicAdd(g + 4 * q, v.x);
+        if (q == 3 && ABS) red_add_v4(g + 4 * q, v.x, v.y, v.z, v.w);   // entry 13 is not 8-byte aligned
+        else if (q == 3) atomicAdd(g + 4 * q, v.x);
         else if (q == 2 && !AUX) red_add_v2(g + 4 * q, v.x, v.y);
         else red_add_v4(g + 4 * q, v.x, v.y, v.z, v.w);
     }
 }
 
 // lane (j, h) sums slot j's moments over half h of the rectangle; after the shuffles it holds the record's quarters
-// 0 and 2 (h == 0) or 1 and 3 (h == 1, quarter 3 with AUX only) and stores them
-template <bool AUX, bool DET, bool OPA>
-__device__ __forceinline__ void bwd_flush(RenderBwdSmem<AUX, DET, OPA>& sm, int warp, int lane, int ns, float cx, float cy,
-                                          float ddelx_dx, float ddely_dy, float* __restrict__ grad_rec) {
+// 0 and 2 (h == 0) or 1 and 3 (h == 1, quarter 3 with AUX or ABS only) and stores them.
+// ABS: the lane also sums, per pixel p, |X_p (A dx_p + B dy_p)| and |X_p (C dy_p + B dx_p)| with d_p = mean2D - pixel,
+// the absolute values of the pixel's signed dL/dmean2D terms before the factors o W/2 and o H/2 (o > 0, applied once
+// at the end); they go to record entries 13 and 14.
+template <bool AUX, bool DET, bool OPA, bool ABS = false>
+__device__ __forceinline__ void bwd_flush(RenderBwdSmem<AUX, DET, OPA, ABS>& sm, int warp, int lane, int ns, float cx,
+                                          float cy, float ddelx_dx, float ddely_dy, float* __restrict__ grad_rec) {
     const int j = lane & (BKS - 1), h = lane >> 4;
     const float2* row = &sm.xw[warp][j][h * 16];
     const float4* dp = &sm.dpix[warp][h * 16];
     float m00 = 0.f, m10 = 0.f, m20 = 0.f, m01 = 0.f, m11 = 0.f, m02 = 0.f;
     float c0 = 0.f, c1 = 0.f, c2 = 0.f, cd = 0.f;
     float x0 = 0.f, x1 = 0.f, x2 = 0.f;
+    float ax = 0.f, ay = 0.f;                    // ABS: the two absolute sums
+    float ca = 0.f, cb = 0.f, cc = 0.f, ex0 = 0.f, ey0 = 0.f;
+    if constexpr (ABS) {
+        // slot j's conic and centre offset (stale for j >= ns: those lanes store nothing)
+        const float4 ga = sm.slot_a[warp][j];
+        ca = ga.z; cb = ga.w; cc = sm.slot_b[warp][j].x;
+        ex0 = ga.x - cx; ey0 = ga.y - cy;
+    }
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
         float r0 = 0.f, r1 = 0.f, r2 = 0.f;
+        float tx0 = 0.f, ty0 = 0.f;              // ABS: A dx + B dy and C dy + B dx at the row's centre column
+        if constexpr (ABS) {
+            const float dyr = ey0 - ((float)(2 * h + rr) - 1.5f);
+            tx0 = fmaf(cb, dyr, ca * ex0);
+            ty0 = fmaf(cb, ex0, cc * dyr);
+        }
 #pragma unroll
         for (int x = 0; x < 8; ++x) {
             const float2 v = row[rr * 8 + x];
             const float4 d = dp[rr * 8 + x];
             const float xc = (float)x - 3.5f;        // pixel x relative to the rectangle centre
+            if constexpr (ABS) {
+                // dx_p = ex0 - xc: the row's terms shifted by -xc along x
+                ax += fabsf(v.x * fmaf(-ca, xc, tx0));
+                ay += fabsf(v.x * fmaf(-cb, xc, ty0));
+            }
             r0 += v.x;
             r1 = fmaf(v.x, xc, r1);
             r2 = fmaf(v.x, xc * xc, r2);
@@ -535,6 +561,9 @@ __device__ __forceinline__ void bwd_flush(RenderBwdSmem<AUX, DET, OPA>& sm, int 
     if (AUX) {
         x0 += __shfl_xor_sync(F, x0, 16); x1 += __shfl_xor_sync(F, x1, 16); x2 += __shfl_xor_sync(F, x2, 16);
     }
+    if (ABS) {
+        ax += __shfl_xor_sync(F, ax, 16); ay += __shfl_xor_sync(F, ay, 16);
+    }
     if (j < ns) {
         const float4 ga = sm.slot_a[warp][j];
         const float4 gb = sm.slot_b[warp][j];
@@ -556,7 +585,9 @@ __device__ __forceinline__ void bwd_flush(RenderBwdSmem<AUX, DET, OPA>& sm, int 
             bwd_store(sm, warp, g, slot, 2, make_float4(c2, cd, x0, x1));   // x0 = x1 = 0 without AUX
         } else {
             bwd_store(sm, warp, g, slot, 1, make_float4(hf * syy, m00, c0, c1));
-            if constexpr (AUX) bwd_store(sm, warp, g, slot, 3, make_float4(x2, 0.f, 0.f, 0.f));
+            if constexpr (ABS)   // x2 = 0 without AUX
+                bwd_store(sm, warp, g, slot, 3, make_float4(x2, o * ddelx_dx * ax, o * ddely_dy * ay, 0.f));
+            else if constexpr (AUX) bwd_store(sm, warp, g, slot, 3, make_float4(x2, 0.f, 0.f, 0.f));
         }
     }
 }
@@ -564,14 +595,15 @@ __device__ __forceinline__ void bwd_flush(RenderBwdSmem<AUX, DET, OPA>& sm, int 
 // OPA: the gradients of the opacity images join the walk.  alpha = 1 - T_final has dalpha/dalpha_i = T_final / (1 -
 // alpha_i), the form of the background term, so T_final dL/dalpha joins nbg; dL/dmedian goes, with weight 1, into the
 // depth sum of the one instance at the pixel's median position.  Both end in the same records as every other term.
-template <bool AUX, bool DET, bool OPA>
+// ABS: the absolute screen-space gradients as well (bwd_flush), in record entries 13 and 14.
+template <bool AUX, bool DET, bool OPA, bool ABS = false>
 __global__ void __launch_bounds__(TILE_PIX)
     render_backward_kernel(std::conditional_t<DET, RenderBwdDetArgs, RenderBwdArgs> args) {
     extern __shared__ __align__(16) unsigned char s_raw[];
-    RenderBwdSmem<AUX, DET, OPA>& sm = *reinterpret_cast<RenderBwdSmem<AUX, DET, OPA>*>(s_raw);
+    RenderBwdSmem<AUX, DET, OPA, ABS>& sm = *reinterpret_cast<RenderBwdSmem<AUX, DET, OPA, ABS>*>(s_raw);
     const RenderBwdArgs& a = args;
-    constexpr int NB = DET ? DCB : BCB;   // instances per staged batch
-    constexpr int NQ = AUX ? 4 : 3;       // record quarters written
+    constexpr int NB = DET ? DCB : BCB;          // instances per staged batch
+    constexpr int NQ = (AUX || ABS) ? 4 : 3;     // record quarters written
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t tile = blockIdx.y * gridDim.x + blockIdx.x;
@@ -750,7 +782,7 @@ __global__ void __launch_bounds__(TILE_PIX)
                     }
                     if (++ns == BKS) {
                         __syncwarp();
-                        bwd_flush(sm, warp, lane, BKS, cx, cy, ddelx_dx, ddely_dy, a.grad_rec);
+                        bwd_flush<AUX, DET, OPA, ABS>(sm, warp, lane, BKS, cx, cy, ddelx_dx, ddely_dy, a.grad_rec);
                         __syncwarp();
                         ns = 0;
                     }
@@ -760,7 +792,7 @@ __global__ void __launch_bounds__(TILE_PIX)
             if constexpr (DET) {
                 if (ns) {
                     __syncwarp();
-                    bwd_flush(sm, warp, lane, ns, cx, cy, ddelx_dx, ddely_dy, a.grad_rec);
+                    bwd_flush<AUX, DET, OPA, ABS>(sm, warp, lane, ns, cx, cy, ddelx_dx, ddely_dy, a.grad_rec);
                     __syncwarp();
                     ns = 0;
                 }
@@ -788,7 +820,7 @@ __global__ void __launch_bounds__(TILE_PIX)
     }
     if (!DET && ns) {
         __syncwarp();
-        bwd_flush(sm, warp, lane, ns, cx, cy, ddelx_dx, ddely_dy, a.grad_rec);
+        bwd_flush<AUX, DET, OPA, ABS>(sm, warp, lane, ns, cx, cy, ddelx_dx, ddely_dy, a.grad_rec);
     }
 }
 
@@ -811,6 +843,18 @@ __global__ void grad_rec_gather_kernel(uint32_t P, int nq, const uint32_t* __res
         }
     }
     grad_rec[(size_t)g * (GRAD_REC / 4) + q] = s;
+}
+
+// dL_dmean2D_abs [P,2] of an absgrad backward: record entries 13 and 14 of the Gaussians with radii > 0, 0 elsewhere
+__global__ void __launch_bounds__(256) absgrad_export_kernel(uint32_t P, const int* __restrict__ radii,
+                                                             const float* __restrict__ grad_rec,
+                                                             float* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P) return;
+    const bool vis = radii[i] > 0;
+    const float* r = grad_rec + (size_t)i * GRAD_REC;
+    out[2 * (size_t)i] = vis ? r[13] : 0.f;
+    out[2 * (size_t)i + 1] = vis ? r[14] : 0.f;
 }
 
 }  // namespace s3g

@@ -113,6 +113,26 @@ __global__ void __launch_bounds__(256) densify_stats_kernel(int P, const float* 
     max_radii[i] = fmaxf(max_radii[i], (float)r);
 }
 
+// densify_stats_kernel plus the absolute-gradient statistic (AbsGS, gsplat absgrad) in the same pass:
+//   xyz_gradient_accum_abs[vis] += |viewspace_absgrad[vis]|   (absgrad f32[P,2])
+__global__ void __launch_bounds__(256) densify_stats_abs_kernel(int P, const float* __restrict__ vgrad,
+                                                               const float* __restrict__ vabs,
+                                                               const int* __restrict__ radii, float* __restrict__ accum,
+                                                               float* __restrict__ accum_abs,
+                                                               float* __restrict__ denom,
+                                                               float* __restrict__ max_radii) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P) return;
+    const int r = radii[i];
+    if (r <= 0) return;
+    const float gx = vgrad[3 * (size_t)i], gy = vgrad[3 * (size_t)i + 1];
+    const float ax = vabs[2 * (size_t)i], ay = vabs[2 * (size_t)i + 1];
+    accum[i] += sqrtf(gx * gx + gy * gy);
+    accum_abs[i] += sqrtf(ax * ax + ay * ay);
+    denom[i] += 1.0f;
+    max_radii[i] = fmaxf(max_radii[i], (float)r);
+}
+
 // ---------------------------------------------------------------------------------------------
 // Image loss terms {mean|x - y|, mean(ssim_map(x, y)), depth_l2} and their gradients,
 // with the reference's SSIM (11x11 Gaussian window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2,

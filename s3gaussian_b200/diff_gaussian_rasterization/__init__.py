@@ -140,19 +140,21 @@ def _camera_inputs(raster_settings):
 
 
 def _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                       raster_settings, colors_aux, opacity):
-    """_RasterizeGaussians.apply of an antialiased forward: every optional input given, antialiasing last."""
+                       raster_settings, colors_aux, opacity, antialiasing=True, absgrad=False):
+    """_RasterizeGaussians.apply of an antialiased or absgrad forward: every optional input given, then the opacity
+    switch, antialiasing and, with absgrad only, absgrad=True last."""
     cam = _camera_inputs(raster_settings)
+    switches = (opacity, bool(antialiasing), True) if absgrad else (opacity, True)
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                      cov3Ds_precomp, raster_settings, colors_aux,
-                                     *(cam if cam is not None else (None, None, None)), opacity, True)
+                                     *(cam if cam is not None else (None, None, None)), *switches)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                        cov3Ds_precomp, raster_settings, antialiasing=False):
-    if antialiasing:
+                        cov3Ds_precomp, raster_settings, antialiasing=False, absgrad=False):
+    if antialiasing or absgrad:
         return _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                  cov3Ds_precomp, raster_settings, None, False)
+                                  cov3Ds_precomp, raster_settings, None, False, antialiasing, absgrad)
     cam = _camera_inputs(raster_settings)
     if cam is not None:
         return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales,
@@ -162,12 +164,12 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales,
 
 
 def rasterize_gaussians_aux(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                            cov3Ds_precomp, raster_settings, colors_aux, antialiasing=False):
+                            cov3Ds_precomp, raster_settings, colors_aux, antialiasing=False, absgrad=False):
     """(color, radii, depth, color_aux): both colour sets composited on ONE preprocess + sort
     (the aux pair of s3g_rasterize_forward / s3g_rasterize_backward)."""
-    if antialiasing:
+    if antialiasing or absgrad:
         return _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                  cov3Ds_precomp, raster_settings, colors_aux, False)
+                                  cov3Ds_precomp, raster_settings, colors_aux, False, antialiasing, absgrad)
     cam = _camera_inputs(raster_settings)
     if cam is not None:
         return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales,
@@ -177,12 +179,12 @@ def rasterize_gaussians_aux(means3D, means2D, sh, colors_precomp, opacities, sca
 
 
 def rasterize_gaussians_opacity(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                cov3Ds_precomp, raster_settings, colors_aux=None, antialiasing=False):
+                                cov3Ds_precomp, raster_settings, colors_aux=None, antialiasing=False, absgrad=False):
     """(color, radii, depth, alpha, median_depth[, color_aux]): the opacity images of s3g_rasterize_forward_opacity
     from the same walk, differentiable like the others (the *_opacity backwards)."""
-    if antialiasing:
+    if antialiasing or absgrad:
         return _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                  cov3Ds_precomp, raster_settings, colors_aux, True)
+                                  cov3Ds_precomp, raster_settings, colors_aux, True, antialiasing, absgrad)
     cam = _camera_inputs(raster_settings)
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                      cov3Ds_precomp, raster_settings, colors_aux,
@@ -287,6 +289,27 @@ def rasterize_gaussians_eval(means3D, means2D, sh, colors_precomp, opacities, sc
 _FUSED_EXCHANGE_WARNED = False
 
 
+def _absgrad_backward_call(lib, scene, bwd, dev, P, H, W, opa, absgrad):
+    """s3g_rasterize_backward_absgrad into `absgrad` (float32 [P,2]): its deterministic form, with a workspace from the
+    caching allocator, under torch.use_deterministic_algorithms(True) as in _backward_call, and its default form with
+    a peer sink (with the same one-time warning)."""
+    global _FUSED_EXCHANGE_WARNED
+    det = torch.are_deterministic_algorithms_enabled()
+    workspace = None
+    if det and not bwd.sink:
+        nbytes = int(lib.s3g_rasterize_backward_deterministic_workspace_bytes(P, bwd.R, W, H))
+        workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev) if nbytes > 0 else None
+    elif det and not _FUSED_EXCHANGE_WARNED:
+        _FUSED_EXCHANGE_WARNED = True
+        warnings.warn("the fused gradient exchange (FusedGradExchange) is not deterministic: the rasterizer "
+                      "backward runs its default, atomic-reduction path while it is installed", UserWarning,
+                      stacklevel=4)
+    _lib.check(lib.s3g_rasterize_backward_absgrad(C.byref(scene), C.byref(bwd), C.byref(opa) if opa is not None
+                                                  else None, absgrad.data_ptr(), 1 if det and not bwd.sink else 0,
+                                                  _ptr(workspace), _stream_ptr(dev)),
+               "rasterize_gaussians_backward_absgrad")
+
+
 def _backward_call(lib, scene, bwd, dev, P, H, W, opa=None):
     """s3g_rasterize_backward, or under torch.use_deterministic_algorithms(True) (warn_only or not) its deterministic
     twin with a workspace from the caching allocator; with `opa` (a RasterOpacityArgs) their *_opacity forms.  The
@@ -339,11 +362,12 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                 cov3Ds_precomp, raster_settings, colors_aux=None, viewmatrix=None, projmatrix=None, campos=None,
-                opacity=False, antialiasing=False):
+                opacity=False, antialiasing=False, absgrad=False):
         # viewmatrix / projmatrix / campos: raster_settings' own tensors, passed (by rasterize_gaussians*) only when
         # one of them requires grad; the backward then returns their gradients.  opacity (rasterize_gaussians_opacity):
         # alpha and median_depth follow depth in the outputs.  antialiasing: s3g_rasterize_forward_antialiased, whose
-        # chain rule the backward calls apply by themselves
+        # chain rule the backward calls apply by themselves.  absgrad: the backward is s3g_rasterize_backward_absgrad
+        # and sets (or adds to) the `absgrad` attribute of the tensor object passed as means2D
         lib = _lib.load()
         rs = raster_settings
         scene, fwd, lease, inputs, color, depth, radii = _forward_args(means3D, sh, colors_precomp, opacities, scales,
@@ -400,6 +424,9 @@ class _RasterizeGaussians(torch.autograd.Function):
             ctx.cam_shapes = (rs.viewmatrix.shape, rs.projmatrix.shape, rs.campos.shape)
         ctx.opacity = bool(opacity)
         ctx.antialiasing = bool(antialiasing)
+        ctx.absgrad = bool(absgrad)
+        if absgrad:
+            ctx.means2D = means2D
         out = (color, radii, depth) + ((alpha, median_depth) if opacity else ()) + ((color_aux,) if has_aux else ())
         return out
 
@@ -408,6 +435,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         # grad_rest: (grad_alpha, grad_median_depth) of an opacity forward, then grad_out_aux with the aux set
         opacity = getattr(ctx, "opacity", False)
         antialiasing = getattr(ctx, "antialiasing", False)
+        absgrad = getattr(ctx, "absgrad", False)
         grad_alpha, grad_median = grad_rest[:2] if opacity else (None, None)
         grad_rest = grad_rest[2:] if opacity else grad_rest
         grad_out_aux = grad_rest[0] if grad_rest else None
@@ -481,16 +509,21 @@ class _RasterizeGaussians(torch.autograd.Function):
                 raise NotImplementedError("FusedGradExchange: an antialiased forward's gradients are not exchanged")
             _GRAD_SINK.note_backward()
             bwd.sink = C.pointer(peer)
+        grad_abs = None
+        call = lambda: _backward_call(lib, scene, bwd, dev, P, H, W, opa)
+        if absgrad:
+            grad_abs = torch.empty((P, 2), dtype=torch.float32, device=dev)     # every row is written
+            call = lambda: _absgrad_backward_call(lib, scene, bwd, dev, P, H, W, opa, grad_abs)
         with torch.cuda.device(dev):
             if P > 0:
                 if rs.debug:
                     try:
-                        _backward_call(lib, scene, bwd, dev, P, H, W, opa)
+                        call()
                     except Exception as ex:
                         print("\nAn error occured in backward.\n")
                         raise ex
                 else:
-                    _backward_call(lib, scene, bwd, dev, P, H, W, opa)
+                    call()
             if any(cam_needs):
                 cam_grads = _camera_backward_call(lib, scene, bwd, dev, P, ctx.cam_shapes, cam_needs)
 
@@ -507,15 +540,22 @@ class _RasterizeGaussians(torch.autograd.Function):
             grad_cov3D if has_cov else None,
             None,
         )
+        if absgrad:
+            # gsplat's means2d.absgrad: set on the tensor object passed as means2D, added to like .grad
+            m2 = ctx.means2D
+            prev = getattr(m2, "absgrad", None)
+            m2.absgrad = grad_abs if prev is None else prev + grad_abs
         if ctx.has_aux:
             grads = grads + (grad_aux,)
-        if ctx.camera or opacity or antialiasing:
+        if ctx.camera or opacity or antialiasing or absgrad:
             if not ctx.has_aux:
                 grads = grads + (None,)
             grads = grads + (cam_grads if any(cam_needs) else (None, None, None))
-        if opacity or antialiasing:
+        if opacity or antialiasing or absgrad:
             grads = grads + (None,)
-        if antialiasing:
+        if antialiasing or absgrad:
+            grads = grads + (None,)
+        if absgrad:
             grads = grads + (None,)
         return grads
 
@@ -553,12 +593,20 @@ class GaussianRasterizer(nn.Module):
     include/s3g_b200.h): each Gaussian's opacity is scaled by h = sqrt(max(det(cov2D) / det(cov2D + 0.3 I), 2.5e-5)),
     so a Gaussian smaller than a pixel keeps its on-screen energy at every resolution.  The backwards, camera
     gradients included, differentiate that forward.  Not in the reference (upstream 3DGS: `antialiasing`, gsplat:
-    rasterize_mode="antialiased")."""
+    rasterize_mode="antialiased").
 
-    def __init__(self, raster_settings, antialiasing=False):
+    absgrad=True: the backwards of forward(), forward_aux() and forward_opacity() also compute each Gaussian's absolute
+    screen-space gradient (AbsGS; gsplat rasterization(absgrad=True)), sum over its pixels p of |dL_p/dmean2D| per
+    component, in the units of means2D.grad, and store it as `means2D.absgrad` (float32 [P,2], zero for Gaussians
+    with radii <= 0) on the tensor object passed as means2D.  A second backward into the same object adds to it, as
+    .grad accumulates; set it to None to start again.  The statistic is per call: the aux pair's two images share one
+    sum, two separate calls add two.  Not in the reference."""
+
+    def __init__(self, raster_settings, antialiasing=False, absgrad=False):
         super().__init__()
         self.raster_settings = raster_settings
         self.antialiasing = bool(antialiasing)
+        self.absgrad = bool(absgrad)
 
     def markVisible(self, positions):
         """bool[P]: passes the near-plane test (rasterizer_impl.cu:54-66)."""
@@ -582,7 +630,7 @@ class GaussianRasterizer(nn.Module):
         shs, colors_precomp, scales, rotations, cov3D_precomp = _reference_inputs(shs, colors_precomp, scales,
                                                                                   rotations, cov3D_precomp)
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales,
-                                   rotations, cov3D_precomp, self.raster_settings, self.antialiasing)
+                                   rotations, cov3D_precomp, self.raster_settings, self.antialiasing, self.absgrad)
 
     def forward_aux(self, means3D, means2D, opacities, colors_aux, shs=None, colors_precomp=None, scales=None,
                     rotations=None, cov3D_precomp=None):
@@ -592,7 +640,8 @@ class GaussianRasterizer(nn.Module):
         shs, colors_precomp, scales, rotations, cov3D_precomp = _reference_inputs(shs, colors_precomp, scales,
                                                                                   rotations, cov3D_precomp)
         return rasterize_gaussians_aux(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                       cov3D_precomp, self.raster_settings, colors_aux, self.antialiasing)
+                                       cov3D_precomp, self.raster_settings, colors_aux, self.antialiasing,
+                                       self.absgrad)
 
     def forward_opacity(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                         cov3D_precomp=None, colors_aux=None):
@@ -605,7 +654,8 @@ class GaussianRasterizer(nn.Module):
         shs, colors_precomp, scales, rotations, cov3D_precomp = _reference_inputs(shs, colors_precomp, scales,
                                                                                   rotations, cov3D_precomp)
         return rasterize_gaussians_opacity(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                           cov3D_precomp, self.raster_settings, colors_aux, self.antialiasing)
+                                           cov3D_precomp, self.raster_settings, colors_aux, self.antialiasing,
+                                           self.absgrad)
 
     def forward_eval(self, means3D, means2D, opacities, group=None, flow_colors=(), shs=None, colors_precomp=None,
                      scales=None, rotations=None, cov3D_precomp=None, with_opacity=False):

@@ -89,7 +89,7 @@ class GradBucket:
         return self.flat
 
 
-def sync_view_stats(viewspace_grad: torch.Tensor, radii: torch.Tensor):
+def sync_view_stats(viewspace_grad: torch.Tensor, radii: torch.Tensor, absgrad: torch.Tensor | None = None):
     """The batch statistics of ONE training step, combined over the ranks' views exactly as the reference
     combines the views of its sequential batch loop: the screen-space gradients ADD
     (train.py:435-437: viewspace_point_tensor_grad += viewspace_point_tensor_list[idx].grad) and the radii take
@@ -97,12 +97,16 @@ def sync_view_stats(viewspace_grad: torch.Tensor, radii: torch.Tensor):
     per-view visibility filters (:392).  Call it ONCE per step on the local per-step tensors (in place), then
     make ONE `GaussianModel.densification_step(viewspace_grad, radii)` call on every rank: the accumulators
     `xyz_gradient_accum` / `denom` / `max_radii2D` themselves are never all-reduced (they would be re-summed
-    every step)."""
+    every step).  `absgrad` (the rasterizer's absolute screen-space gradient, summed over the rank's views) ADDS like
+    the signed gradient; when given it is synchronised too and returned third."""
+    out = (viewspace_grad, radii) if absgrad is None else (viewspace_grad, radii, absgrad)
     if not (dist.is_initialized() and dist.get_world_size() > 1):
-        return viewspace_grad, radii
+        return out
     dist.all_reduce(viewspace_grad, op=dist.ReduceOp.SUM)
     dist.all_reduce(radii, op=dist.ReduceOp.MAX)
-    return viewspace_grad, radii
+    if absgrad is not None:
+        dist.all_reduce(absgrad, op=dist.ReduceOp.SUM)
+    return out
 
 
 def broadcast_gaussians(tensors: dict, src: int = 0) -> dict:

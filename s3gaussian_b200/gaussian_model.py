@@ -27,6 +27,12 @@ Not in the reference: Mip-Splatting's 3-D smoothing filter (filter3d.py).  ``com
 ``pipe.filter_3d``.  Densify, prune and ``spatial_sort`` carry it (a new row takes its source row's value) until the
 loop recomputes it.  It is not saved: ``capture()`` / ``restore()`` and the .ply files keep the reference's layout, so
 recompute it from the training cameras after loading.
+
+Not in the reference either: the absolute screen-space gradient statistic (AbsGS; gsplat ``DefaultStrategy(absgrad=True)``).
+``densification_step(grad, radii, absgrad)`` also accumulates ``||absgrad||`` into ``xyz_gradient_accum_abs`` [P,1],
+which prune and ``spatial_sort`` carry and densify resets like ``xyz_gradient_accum``; ``densify(..., max_grad_abs=T)``
+then selects clones and splits on ``||xyz_gradient_accum_abs / denom|| >= T``.  It is not saved: ``capture()`` keeps the
+reference's 14-tuple and ``restore()`` starts the accumulator from zero.
 """
 from __future__ import annotations
 
@@ -95,6 +101,7 @@ class GaussianModel:
         e = torch.empty(0)
         self._xyz = self._features_dc = self._features_rest = self._scaling = self._rotation = self._opacity = e
         self.max_radii2D = self.xyz_gradient_accum = self.denom = self._deformation_accum = e
+        self.xyz_gradient_accum_abs = e
         self._deformation_table = e
         self.filter_3D = e              # [P,1] once compute_3D_filter() ran; empty until then
         self.optimizer = None
@@ -247,6 +254,7 @@ class GaussianModel:
         P = self._xyz.shape[0]
         self.percent_dense = training_args.percent_dense
         self.xyz_gradient_accum = torch.zeros((P, 1), device=dev)
+        self.xyz_gradient_accum_abs = torch.zeros((P, 1), device=dev)
         self.denom = torch.zeros((P, 1), device=dev)
         self._deformation_accum = torch.zeros((P, 3), device=dev)
         s = self.spatial_lr_scale
@@ -308,7 +316,7 @@ class GaussianModel:
         self.max_radii2D = max_radii2D.to(dev)
         self._deformation = self._deformation.to(dev)
         self._deformation.load_state_dict(deform_state)
-        self.training_setup(training_args)
+        self.training_setup(training_args)     # xyz_gradient_accum_abs, not in the tuple, starts from zero
         self.xyz_gradient_accum = xyz_gradient_accum.to(dev)
         self.denom = denom.to(dev)
         self.optimizer.load_state_dict(opt_dict)
@@ -319,10 +327,15 @@ class GaussianModel:
         add_densification_stats(viewspace_point_tensor.contiguous(), update_filter.to(torch.int32), self.xyz_gradient_accum,
                                 self.denom, scratch)
 
-    def densification_step(self, viewspace_point_tensor_grad, radii):
-        """max_radii2D update + add_densification_stats with visibility_filter = radii > 0, one launch."""
+    def densification_step(self, viewspace_point_tensor_grad, radii, absgrad=None):
+        """max_radii2D update + add_densification_stats with visibility_filter = radii > 0, one launch.  absgrad
+        (float32 [P,2], viewspace_points.absgrad summed over the step's views) also goes into xyz_gradient_accum_abs."""
+        if absgrad is None:
+            add_densification_stats(viewspace_point_tensor_grad.contiguous(), radii, self.xyz_gradient_accum,
+                                    self.denom, self.max_radii2D)
+            return
         add_densification_stats(viewspace_point_tensor_grad.contiguous(), radii, self.xyz_gradient_accum, self.denom,
-                                self.max_radii2D)
+                                self.max_radii2D, absgrad.contiguous(), self.xyz_gradient_accum_abs)
 
     # ---- row surgery --------------------------------------------------------------------------------
     def _group(self, name):
@@ -366,6 +379,9 @@ class GaussianModel:
         if keep_accumulators:
             acc = [add(self.xyz_gradient_accum, False), add(self.denom, False), add(self._deformation_accum, False),
                    add(self.max_radii2D.unsqueeze(1), False)]
+            # the absolute-gradient accumulator, when it matches the rows (zeros otherwise)
+            acc_abs = self.xyz_gradient_accum_abs
+            acc.append(add(acc_abs, False) if acc_abs.dim() == 2 and acc_abs.shape[0] == P_old else None)
         if n_out > 0:
             arr = (_lib.RowTensor * len(descs))(*descs)
             _lib.check(lib.s3g_gather_rows(len(descs), arr, n_out, int(n_kept), src_index.data_ptr(),
@@ -386,8 +402,10 @@ class GaussianModel:
         if keep_accumulators:
             self.xyz_gradient_accum, self.denom, self._deformation_accum = acc[0], acc[1], acc[2]
             self.max_radii2D = acc[3].squeeze(1)
+            self.xyz_gradient_accum_abs = acc[4] if acc[4] is not None else torch.zeros((n_out, 1), device=dev)
         else:       # densification_postfix resets them (gaussian_model.py:490-494)
             self.xyz_gradient_accum = torch.zeros((n_out, 1), device=dev)
+            self.xyz_gradient_accum_abs = torch.zeros((n_out, 1), device=dev)
             self._deformation_accum = torch.zeros((n_out, 3), device=dev)
             self.denom = torch.zeros((n_out, 1), device=dev)
             self.max_radii2D = torch.zeros(n_out, device=dev)
@@ -462,9 +480,13 @@ class GaussianModel:
             self._xyz.data[n_kept:] = new_xyz
             self._scaling.data[n_kept:] = new_scaling
 
-    def densify(self, max_grad, min_opacity, extent, max_screen_size, *unused, **unused_kw):
-        """gaussian_model.py:674-679."""
-        grads = self.xyz_gradient_accum / self.denom
+    def densify(self, max_grad, min_opacity, extent, max_screen_size, *unused, max_grad_abs=None, **unused_kw):
+        """gaussian_model.py:674-679.  max_grad_abs: clone and split select on the absolute-gradient statistic,
+        ||xyz_gradient_accum_abs / denom|| >= max_grad_abs, instead of the signed one (gsplat's absgrad rule)."""
+        if max_grad_abs is None:
+            grads = self.xyz_gradient_accum / self.denom
+        else:
+            grads, max_grad = self.xyz_gradient_accum_abs / self.denom, max_grad_abs
         grads[grads.isnan()] = 0.0
         with torch.no_grad():
             self.densify_and_clone(grads, max_grad, extent)

@@ -78,6 +78,7 @@ class PipelineParams:       # arguments/__init__.py:93-98 defaults
     render_opacity = False  # ours: render() also returns the alpha and median-depth images (and alpha_d / alpha_s)
     antialiasing = False    # ours: the rasterizer's antialiasing filter (GaussianRasterizer(antialiasing=True))
     filter_3d = False       # ours: Mip-Splatting's 3-D smoothing filter on the scales and opacities (pc.filter_3D)
+    absgrad = False         # ours: the backward also sets viewspace_points.absgrad (GaussianRasterizer(absgrad=True))
 
 
 def pipe_shared_binning(pipe) -> bool:
@@ -89,8 +90,12 @@ def pipe_render_opacity(pipe) -> bool:
 
 
 def pipe_rasterizer_kwargs(pipe) -> dict:
-    """The keyword arguments GaussianRasterizer takes from the pipeline parameters: none unless pipe.antialiasing."""
-    return {"antialiasing": True} if getattr(pipe, "antialiasing", False) else {}
+    """The keyword arguments GaussianRasterizer takes from the pipeline parameters: none unless pipe.antialiasing or
+    pipe.absgrad is set."""
+    kw = {"antialiasing": True} if getattr(pipe, "antialiasing", False) else {}
+    if getattr(pipe, "absgrad", False):
+        kw["absgrad"] = True
+    return kw
 
 
 def pipe_filter_3d(pipe, pc) -> bool:
@@ -111,7 +116,11 @@ def pipe_filter_3d(pipe, pc) -> bool:
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
            stage="fine", return_decomposition=False, return_dx=False, render_feat=False):
-    """Render the scene.  Background tensor (bg_color) must be on GPU!"""
+    """Render the scene.  Background tensor (bg_color) must be on GPU!
+
+    With pipe.absgrad, the backward of the result also sets result["viewspace_points"].absgrad (float32 [P,2]), the
+    absolute screen-space gradient of the call(s) that drew "render" and "feat" (GaussianRasterizer(absgrad=True)).
+    The differentiable decomposition passes index means2D and leave their statistic on those temporaries."""
     filter_3d = pipe_filter_3d(pipe, pc)
     xyz = pc.get_xyz
     dev = xyz.device

@@ -89,17 +89,35 @@ class FusedAdam(torch.optim.Optimizer):
 
 
 def add_densification_stats(viewspace_grad: torch.Tensor, radii: torch.Tensor, xyz_gradient_accum: torch.Tensor,
-                            denom: torch.Tensor, max_radii2D: torch.Tensor) -> None:
+                            denom: torch.Tensor, max_radii2D: torch.Tensor, viewspace_absgrad: torch.Tensor | None = None,
+                            xyz_gradient_accum_abs: torch.Tensor | None = None) -> None:
     """train.py:489-491 in one launch: for ``radii > 0`` update ``max_radii2D`` and call
-    ``GaussianModel.add_densification_stats`` (scene/gaussian_model.py:693-695).  In place."""
+    ``GaussianModel.add_densification_stats`` (scene/gaussian_model.py:693-695).  In place.
+    With ``viewspace_absgrad`` (float32 [P,2], the rasterizer's absgrad) and ``xyz_gradient_accum_abs`` [P,1], both or
+    neither, the same launch also adds ``||viewspace_absgrad||`` to ``xyz_gradient_accum_abs`` (s3g_densify_stats_abs)."""
     P = radii.shape[0]
-    for t in (viewspace_grad, radii, xyz_gradient_accum, denom, max_radii2D):
+    if (viewspace_absgrad is None) != (xyz_gradient_accum_abs is None):
+        raise RuntimeError("add_densification_stats: viewspace_absgrad and xyz_gradient_accum_abs go together")
+    extra = () if viewspace_absgrad is None else (viewspace_absgrad, xyz_gradient_accum_abs)
+    for t in (viewspace_grad, radii, xyz_gradient_accum, denom, max_radii2D) + extra:
         if not t.is_cuda or not t.is_contiguous():
             raise RuntimeError("add_densification_stats: contiguous CUDA tensors only (there is no CPU path)")
     if radii.dtype != torch.int32 or viewspace_grad.dtype != torch.float32 or viewspace_grad.shape != (P, 3):
         raise RuntimeError("add_densification_stats: radii int32 [P], viewspace_grad float32 [P,3]")
     if xyz_gradient_accum.numel() != P or denom.numel() != P or max_radii2D.numel() != P:
         raise RuntimeError("add_densification_stats: accumulator sizes do not match P")
+    if extra:
+        if viewspace_absgrad.dtype != torch.float32 or viewspace_absgrad.shape != (P, 2):
+            raise RuntimeError("add_densification_stats: viewspace_absgrad float32 [P,2]")
+        if xyz_gradient_accum_abs.dtype != torch.float32 or xyz_gradient_accum_abs.numel() != P:
+            raise RuntimeError("add_densification_stats: xyz_gradient_accum_abs float32 with P elements")
+        _lib.check(_lib.load().s3g_densify_stats_abs(P, viewspace_grad.data_ptr(), viewspace_absgrad.data_ptr(),
+                                                     radii.data_ptr(), xyz_gradient_accum.data_ptr(),
+                                                     xyz_gradient_accum_abs.data_ptr(), denom.data_ptr(),
+                                                     max_radii2D.data_ptr(),
+                                                     C.c_void_p(torch.cuda.current_stream().cuda_stream)),
+                   "s3g_densify_stats_abs")
+        return
     _lib.check(_lib.load().s3g_densify_stats(P, viewspace_grad.data_ptr(), radii.data_ptr(),
                                              xyz_gradient_accum.data_ptr(), denom.data_ptr(), max_radii2D.data_ptr(),
                                              C.c_void_p(torch.cuda.current_stream().cuda_stream)),
