@@ -705,7 +705,8 @@ int s3g_image_l1_depth_backward(int B, int C, int H, int W, const float* image, 
  * s3g_plane_reg_*  <- GaussianModel.compute_regulation                 scene/gaussian_model.py:710-749
  *                     + compute_plane_smoothness                        scene/regulation.py:22-28
  * total = sum_planes  w_smooth * mean((t[h+2]-2t[h+1]+t[h])^2 over [1,C,H-2,W]) + w_l1 * mean|1-t|
- * Each plane is the [1,C,H,W] tensor stored channels-last, i.e. physically [H][W][C]; C % 4 == 0, H >= 3.
+ * Each plane is the [1,C,H,W] tensor stored channels-last, i.e. physically [H][W][C]; C % 4 == 0, H >= 3;
+ * plane and grad pointers 16-byte aligned (S3G_ERR_ARG before any launch otherwise).
  * `planes` is a HOST array (device pointers inside), n <= 48.  forward: total = DEVICE double[1],
  * workspace of s3g_plane_reg_workspace_bytes(...) bytes.  backward: gscale = DEVICE float[1] (the
  * upstream gradient); OVERWRITES planes[i].grad (same physical layout) with gscale * d total/d plane. */

@@ -231,6 +231,9 @@ int reg_table(int n, const s3g_plane_desc* planes, bool need_grad, RegArgs& a) {
         const s3g_plane_desc& d = planes[i];
         if (!d.plane || (need_grad && !d.grad)) return fail(S3G_ERR_ARG, "plane_reg: null plane / grad pointer");
         if (d.H < 3 || d.W < 1 || d.C < 4 || d.C % 4) return fail(S3G_ERR_ARG, "plane_reg: need H >= 3, W >= 1, C % 4 == 0");
+        // the kernels read planes and write gradients as float4
+        if ((reinterpret_cast<uintptr_t>(d.plane) | (need_grad ? reinterpret_cast<uintptr_t>(d.grad) : 0)) & 15)
+            return fail(S3G_ERR_ARG, "plane_reg: plane / grad pointers must be 16-byte aligned");
         RegPlane& p = a.p[i];
         p.t = d.plane; p.g = d.grad; p.H = d.H; p.W = d.W; p.C = d.C;
         p.k_smooth = (float)((double)d.w_smooth / ((double)d.C * (d.H - 2) * d.W));

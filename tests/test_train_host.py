@@ -103,6 +103,65 @@ def test_gather_rows_argument_checks(built_lib):
     assert lib.s3g_gather_rows(1, t, 0, 0, None, None) == 0           # nothing to do
 
 
+def test_image_loss_argument_checks(built_lib):
+    """Every call below is refused before any launch; the fake device addresses are never dereferenced."""
+    from s3gaussian_b200 import _lib
+    lib = _lib.load()
+    P = 256
+    for fwd in (lib.s3g_image_loss_forward, lib.s3g_image_l1_depth_forward):
+        assert fwd(1, 65536, 4, 4, P, P, None, None, 80.0, P, P, None) == -1      # B*C = 65536 planes
+        assert fwd(65536, 1, 4, 4, P, P, None, None, 80.0, P, P, None) == -1
+        assert fwd(1, 0, 4, 4, None, None, None, None, 80.0, P, P, None) == -1    # C = 0 and no depth
+        assert fwd(1, 3, 4, 4, P, P, P, None, 80.0, P, P, None) == -1             # depth without gt_depth
+        assert fwd(1, 3, 4, 4, P, P, None, P, 80.0, P, P, None) == -1             # gt_depth without depth
+        assert fwd(1, 3, 4, 4, None, P, None, None, 80.0, P, P, None) == -1       # C > 0 and no image
+        assert fwd(1, 3, 0, 4, P, P, None, None, 80.0, P, P, None) == -1          # empty image
+        assert fwd(1, 3, 4, 4, P, P, None, None, 80.0, None, P, None) == -1       # no sums
+        assert fwd(1, 3, 4, 4, P, P, None, None, 80.0, P, None, None) == -1       # no workspace
+    bwd = lib.s3g_image_loss_backward
+    assert bwd(1, 65536, 4, 4, P, P, None, None, 80.0, P, P, P, P, None, None) == -1
+    assert bwd(1, 0, 4, 4, None, None, None, None, 80.0, P, P, P, None, None, None) == -1
+    assert bwd(1, 3, 4, 4, P, P, P, None, 80.0, P, P, P, P, P, None) == -1
+    assert bwd(1, 3, 4, 4, P, P, None, None, 80.0, P, P, P, None, None, None) == -1     # no g_image
+    assert bwd(1, 0, 4, 4, None, None, P, P, 80.0, P, P, P, None, None, None) == -1     # no g_depth
+    bl1 = lib.s3g_image_l1_depth_backward
+    assert bl1(1, 65536, 4, 4, P, P, None, None, 80.0, P, P, P, None, None) == -1
+    assert bl1(1, 0, 4, 4, None, None, None, None, 80.0, P, P, None, None, None) == -1
+    assert bl1(1, 3, 4, 4, P, P, None, P, 80.0, P, P, P, None, None) == -1
+    assert bl1(1, 3, 4, 4, P, P, None, None, 80.0, None, P, P, None, None) == -1       # no weights
+    # the largest plane count is accepted (sizing only; nothing runs)
+    assert lib.s3g_image_loss_workspace_bytes(65535, 1, 1, 1) > 0
+    assert lib.s3g_image_loss_workspace_bytes(1, 3, 0, 4) == 0
+
+
+def test_plane_reg_argument_checks(built_lib):
+    """The 48-plane table limit, H >= 3, C % 4 == 0 and 16-byte alignment are checked before any launch; the
+    workspace holds one double per 1024-float4 block."""
+    from s3gaussian_b200 import _lib
+    lib = _lib.load()
+    P, G = 256, 512
+
+    def table(*shapes, plane=P, grad=G):
+        return (_lib.PlaneDesc * len(shapes))(*[_lib.PlaneDesc(plane, grad, H, W, Cc, 1.0, 0.5) for H, W, Cc in shapes])
+    ok = table(*[(4, 2, 4)] * 48)
+    assert lib.s3g_plane_reg_workspace_bytes(48, ok) == 256 + 8 * 48
+    for n, t in ((49, table(*[(4, 2, 4)] * 49)), (0, ok), (1, table((2, 8, 4))), (1, table((3, 8, 6))),
+                 (1, table((3, 8, 2))), (1, table((3, 0, 4))), (1, table((3, 8, 4), plane=P + 4))):
+        assert lib.s3g_plane_reg_workspace_bytes(n, t) == 0
+        assert lib.s3g_plane_reg_forward(n, t, P, P, None) == -1
+        assert lib.s3g_plane_reg_backward(n, t, P, None) == -1
+    unaligned_grad = table((3, 8, 4), grad=G + 8)
+    assert lib.s3g_plane_reg_workspace_bytes(1, unaligned_grad) > 0     # the forward reads no gradient
+    assert lib.s3g_plane_reg_backward(1, unaligned_grad, P, None) == -1
+    assert lib.s3g_plane_reg_backward(1, table((3, 8, 4), grad=None), P, None) == -1
+    assert lib.s3g_plane_reg_backward(1, table((3, 8, 4)), None, None) == -1           # no upstream gradient
+    assert lib.s3g_plane_reg_forward(1, table((3, 8, 4)), None, P, None) == -1         # no total
+    # blocks of 1024 float4: 1023 and 1024 float4 fit one block, 1025 take two
+    for H, blocks in ((1023, 1), (1024, 1), (1025, 2)):
+        assert lib.s3g_plane_reg_workspace_bytes(1, table((H, 1, 4))) == 256 + 8 * blocks
+    assert lib.s3g_plane_reg_workspace_bytes(2, table((1025, 1, 4), (7, 300, 8))) == 256 + 8 * (2 + 5)
+
+
 def test_peer_slices_cover_the_buffer_in_float4_units():
     from s3gaussian_b200.dp import peer_slices
     for numel, world in ((40, 3), (8, 8), (118_000_000, 8), (4, 2), (472, 5)):

@@ -9,6 +9,10 @@
   stats case : the two statements of train.py:489-491 executed verbatim around the reference's own
                GaussianModel.add_densification_stats, whose source is extracted from
                scene/gaussian_model.py with ast (the module itself needs simple_knn/open3d to import).
+
+np.savez_compressed stamps each member with the time of writing, so a rerun changes the bytes of files whose values
+are unchanged: to add a case, pass a scratch directory as the argument and copy only the new case's file into
+tests/golden.
 """
 import ast
 import os
@@ -27,6 +31,11 @@ LOSS_CASES = [
     ("batch2", 2, 3, 64, 96, 12),
     ("tiny", 1, 3, 7, 9, 13),          # smaller than the 11x11 window
     ("tile_edges", 1, 3, 65, 33, 14),  # one pixel past a 32x32 tile in both directions
+    ("gray", 1, 1, 23, 29, 15),        # C = 1: one plane per image
+    ("c4_batch3", 3, 4, 19, 35, 16),   # C = 4, B = 3: 12 planes
+    ("window", 1, 3, 11, 11, 17),      # exactly the 11x11 window
+    ("row", 1, 3, 1, 40, 18),          # a single row: every window tap but the centre row is padding
+    ("tile_cross", 2, 3, 33, 97, 19),  # past one tile vertically and two horizontally, 6 planes
 ]
 
 
