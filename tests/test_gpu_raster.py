@@ -131,6 +131,14 @@ def test_cuda_matches_reference_extension_at_benchmark_sizes(P, W, H, mode, view
     cloud = syn.make_cloud(P, seed=0)
     cam = syn.make_camera(W, H, (0, 0, 2.0)) if view == "front" else bench_camera(W, H, 0)
     d = util.scene_inputs(cloud, cam, mode=mode, sh_degree=3, bg=(0.0, 0.0, 0.0))
+    check_against_reference_extension(ref, ours, d, f"P={P} {mode} {view}")
+
+
+def check_against_reference_extension(ref, ours, d, label):
+    """The same scene dict through both implementations: integer state bit-exact, images within 1e-4 of the tensor
+    max and element-wise, gradients within 1e-4 as means of 4 runs and element-wise above the reference's own
+    run-to-run spread."""
+    P, W, H = d["means3D"].shape[0], d["W"], d["H"]
     gc, gd = util.seeded_grads(d, 7)
     # Both backward passes accumulate per-Gaussian gradients with unordered fp32 atomics, so two runs of the SAME
     # implementation differ: at 2.6 M the reference differs from itself by 1.3e-4 of the tensor max on the rotation
@@ -162,7 +170,7 @@ def test_cuda_matches_reference_extension_at_benchmark_sizes(P, W, H, mode, view
         # on this input, 1e-6 of the tensor max)
         atol = max(4.0 * spread, 1e-6 * tmax)
         frac, worst, idx = util.elementwise(a, b, 1e-4, atol)
-        print(f"[elementwise] P={P} {mode} {view} {k}: max-normalised {e:.2e} (means of {NRUN} runs: {e_mean:.2e}), "
+        print(f"[elementwise] {label} {k}: max-normalised {e:.2e} (means of {NRUN} runs: {e_mean:.2e}), "
               f"atol {atol:.2e} (ref spread {spread:.2e}, tensor max {tmax:.2e}), "
               f"outside {frac:.2e}, worst ratio {worst:.2f}")
         assert frac <= 1e-6, (k, frac, worst, idx)
@@ -171,9 +179,9 @@ def test_cuda_matches_reference_extension_at_benchmark_sizes(P, W, H, mode, view
     E = torch.Tensor([])
     g = lambda k: d[k].to(DEV).contiguous() if d[k] is not None else E
     R0, _, _, _, gb, bb, ib = ref._C.rasterize_gaussians(
-        d["bg"].to(DEV), g("means3D"), g("colors_precomp"), g("opacities"), g("scales"), g("rotations"), 1.0,
-        g("cov3D_precomp"), d["viewmatrix"].to(DEV), d["projmatrix"].to(DEV), d["tanfovx"], d["tanfovy"], H, W,
-        g("shs"), 3, d["campos"].to(DEV), False, False)
+        d["bg"].to(DEV), g("means3D"), g("colors_precomp"), g("opacities"), g("scales"), g("rotations"),
+        d.get("scale_modifier", 1.0), g("cov3D_precomp"), d["viewmatrix"].to(DEV), d["projmatrix"].to(DEV),
+        d["tanfovx"], d["tanfovy"], H, W, g("shs"), d["sh_degree"], d["campos"].to(DEV), False, False)
     torch.cuda.synchronize()
     rg, rb, ri = ref_ext.decode_geom(gb, P), ref_ext.decode_binning(bb, R0), ref_ext.decode_image(ib, W * H)
     del gb, bb, ib

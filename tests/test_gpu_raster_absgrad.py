@@ -75,7 +75,13 @@ def _absgrad_run(ours, d, dL, aa, det, aux_cols=None, m2d=None):
 @pytest.mark.parametrize("loss_kind", list(LOSSES))
 @pytest.mark.parametrize("P,W,H,seed,cov", SHAPES)
 def test_absgrad_matches_float64_oracle(P, W, H, seed, cov, loss_kind, aa, det, ours):
-    d = _grad_case(P, W, H, seed, cov)
+    check_absgrad_against_restatement(ours, _grad_case(P, W, H, seed, cov), seed, loss_kind, aa, det)
+
+
+def check_absgrad_against_restatement(ours, d, seed, loss_kind, aa, det):
+    """means2D.absgrad of forward_opacity(absgrad=True) for `loss_kind` against absgrad_ref in float64; d holds
+    precomputed colours."""
+    P, W, H, cov = d["means3D"].shape[0], d["W"], d["H"], d["cov3D_precomp"] is not None
     _, _, _, _, lists = util.ours_forward_state(d, DEV)
     gen = torch.Generator().manual_seed(seed + 200)
     dL = {k: torch.randn(3 if k in ("color", "aux") else 1, H, W, generator=gen, dtype=torch.float64)

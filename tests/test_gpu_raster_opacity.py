@@ -315,7 +315,13 @@ LOSSES = ["alpha", "median", "all"]
 @pytest.mark.parametrize("loss_kind", LOSSES)
 @pytest.mark.parametrize("P,W,H,seed,cov", [(48, 48, 40, 3, False), (64, 40, 33, 5, True), (32, 64, 32, 9, False)])
 def test_gradients_match_float64_restatement(P, W, H, seed, cov, loss_kind, ours):
-    d = _grad_case(P, W, H, seed, cov)
+    check_gradients_against_restatement(ours, _grad_case(P, W, H, seed, cov), seed, loss_kind)
+
+
+def check_gradients_against_restatement(ours, d, seed, loss_kind):
+    """forward_opacity's gradients (Gaussians and camera) for `loss_kind` against _restated_images in float64; d holds
+    precomputed colours."""
+    P, W, H, cov = d["means3D"].shape[0], d["W"], d["H"], d["cov3D_precomp"] is not None
     _, _, _, _, lists = util.ours_forward_state(d, DEV)
     gen = torch.Generator().manual_seed(seed + 100)
     gc, gd, ga, gm = (torch.randn(ch, H, W, generator=gen, dtype=torch.float64) for ch in (3, 1, 1, 1))

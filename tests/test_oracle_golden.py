@@ -23,6 +23,8 @@ def load_case(path):
         d[k] = int(z["in_" + k])
     for k in ("tanfovx", "tanfovy"):
         d[k] = float(z["in_" + k])
+    if "in_scale_modifier" in z.files:
+        d["scale_modifier"] = float(z["in_scale_modifier"])
     return z, d
 
 

@@ -1,6 +1,8 @@
 """Shared helpers for the parity tests (test infrastructure)."""
 from __future__ import annotations
 
+import math
+
 import numpy as np
 import torch
 
@@ -36,10 +38,21 @@ def cov3d_from(scales, rot):
     return torch.stack([S[:, 0, 0], S[:, 0, 1], S[:, 0, 2], S[:, 1, 1], S[:, 1, 2], S[:, 2, 2]], 1).float()
 
 
+def anisotropic_camera(W, H, fx, fy, position, yaw_deg=0.0):
+    """A camera posed like synthetic.make_camera(W, H, position, yaw_deg) whose focal lengths differ: FoVx from fx,
+    FoVy from fy (the reference's Waymo reader scales fx and fy separately, so they are equal only by chance)."""
+    base = syn.make_camera(W, H, position, yaw_deg=yaw_deg, focal=fx)
+    fovx, fovy = 2 * math.atan(W / (2 * fx)), 2 * math.atan(H / (2 * fy))
+    wvt = base.world_view_transform
+    proj = syn.projection_matrix(syn.ZNEAR, syn.ZFAR, fovx, fovy).transpose(0, 1)
+    full = (wvt.unsqueeze(0).bmm(proj.unsqueeze(0))).squeeze(0).contiguous()
+    return syn.SyntheticCamera(W, H, fovx, fovy, wvt, full, base.camera_center, base.time)
+
+
 def settings_for(mod, d, dev, debug=False):
     return mod.GaussianRasterizationSettings(
         image_height=d["H"], image_width=d["W"], tanfovx=d["tanfovx"], tanfovy=d["tanfovy"],
-        bg=d["bg"].to(dev), scale_modifier=1.0, viewmatrix=d["viewmatrix"].to(dev),
+        bg=d["bg"].to(dev), scale_modifier=d.get("scale_modifier", 1.0), viewmatrix=d["viewmatrix"].to(dev),
         projmatrix=d["projmatrix"].to(dev), sh_degree=d["sh_degree"], campos=d["campos"].to(dev),
         prefiltered=False, debug=debug)
 
@@ -126,7 +139,7 @@ def oracle_run(oracle_mod, d, grad_color=None, grad_depth=None):
         viewmatrix=d["viewmatrix"].numpy(), projmatrix=d["projmatrix"].numpy(), campos=d["campos"].numpy(),
         tanfovx=d["tanfovx"], tanfovy=d["tanfovy"], sh_degree=d["sh_degree"], shs=n("shs"),
         colors_precomp=n("colors_precomp"), scales=n("scales"), rotations=n("rotations"),
-        cov3D_precomp=n("cov3D_precomp"))
+        cov3D_precomp=n("cov3D_precomp"), scale_modifier=d.get("scale_modifier", 1.0))
     out = dict(color=color, radii=radii, depth=depth, R=o.R, geometry=o.geometry(), binning=o.binning(),
                image=o.image_state(), grads=None)
     if grad_color is not None:
