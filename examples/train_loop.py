@@ -2,7 +2,7 @@
 train.py (scene_reconstruction, train.py:330-530) with every heavy step running through libs3g_b200.so.
 
     python examples/train_loop.py [--points 200000] [--iters 300] [--fine] [--filter-3d] [--densify-until N]
-                                 [--absgrad-threshold T]
+                                 [--absgrad-threshold T | --mcmc-cap N]
 
 Synthetic data (there is no dataset reader here): a random cloud initialised through create_from_pcd
 (3-NN scales), targets rendered from a perturbed copy of it.  Needs a CUDA device (sm_90a).
@@ -35,7 +35,12 @@ def main():
     ap.add_argument("--absgrad-threshold", type=float, default=0.0,
                     help="densify on the absolute screen-space gradient (AbsGS, gsplat absgrad) with this threshold "
                          "instead of the signed one (0: off)")
+    ap.add_argument("--mcmc-cap", type=int, default=0,
+                    help="3DGS-MCMC densification up to this many Gaussians instead of densify / prune: relocation, "
+                         "5 %% growth per interval, position noise and the opacity / scale regularisers (0: off)")
     a = ap.parse_args()
+    if a.mcmc_cap and a.absgrad_threshold > 0:
+        ap.error("--mcmc-cap replaces densify / prune, so --absgrad-threshold has nothing to select")
     if not torch.cuda.is_available():
         raise SystemExit("needs a CUDA device: s3gaussian_b200 has no CPU path")
     dev = torch.device("cuda:0")
@@ -78,7 +83,7 @@ def main():
     for it in range(1, a.iters + 1):
         if it == 11:
             e0.record()
-        gaussians.update_learning_rate(it)
+        xyz_lr = gaussians.update_learning_rate(it)
         if it % 100 == 0:
             gaussians.oneupSHdegree()
         k = (it - 1) % len(cams)
@@ -89,12 +94,20 @@ def main():
         if a.fine:
             loss = loss + 0.001 * out["dx"].abs().mean() + 0.001 * out["dshs"].abs().mean() + \
                 gaussians.compute_regulation(0.01, 0.0001, 0.0001)
+        if a.mcmc_cap:      # 3DGS-MCMC's opacity and scale regularisers (its train.py, opacity_reg = scale_reg = 0.01)
+            loss = loss + 0.01 * gaussians.get_opacity.mean() + 0.01 * gaussians.get_scaling.mean()
         loss.backward()
         with torch.no_grad():
             vs = out["viewspace_points"]
             gaussians.densification_step(vs.grad, out["radii"], getattr(vs, "absgrad", None))   # train.py:489-491
             densifying = not a.densify_until or it < a.densify_until
-            if densifying and it > 50 and it % 100 == 0:
+            if a.mcmc_cap and densifying and it > 50 and it % 100 == 0:
+                gaussians.relocate_gs()
+                gaussians.add_new_gs(a.mcmc_cap)
+                gaussians.spatial_sort()
+                if a.filter_3d:
+                    gaussians.compute_3D_filter(cams)
+            elif densifying and it > 50 and it % 100 == 0:
                 gaussians.densify(0.0002, 0.005, extent, 20 if it > 3000 else None,
                                   max_grad_abs=a.absgrad_threshold if a.absgrad_threshold > 0 else None)
                 gaussians.prune(0.0002, 0.005, extent, 20 if it > 3000 else None)
@@ -105,6 +118,8 @@ def main():
                 gaussians.compute_3D_filter(cams)         # then every 100 iterations, except near the end
         gaussians.optimizer.step()                                               # one launch over all groups
         gaussians.optimizer.zero_grad(set_to_none=True)
+        if a.mcmc_cap:
+            gaussians.inject_noise(xyz_lr)
         if it % 50 == 0:
             print(f"iter {it:5d}  loss {loss.item():.5f}  l1 {l1.item():.5f}  ssim {ssim_value.item():.4f}  "
                   f"points {gaussians.get_xyz.shape[0]}")

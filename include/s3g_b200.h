@@ -736,6 +736,43 @@ typedef struct s3g_row_tensor {
 int s3g_gather_rows(int n, const s3g_row_tensor* tensors, int64_t n_out, int64_t n_kept, const int64_t* src_index,
                     void* stream);
 
+/* ---- MCMC densification (3DGS-MCMC, Kheradmand et al. 2024; gsplat MCMCStrategy) ---------------------------------
+ * Not in the reference, whose densification is the clone / split / prune heuristics.  3DGS-MCMC replaces them with
+ * relocating near-transparent Gaussians onto live ones, growing to a fixed budget, and position noise.
+ *
+ * s3g_mcmc_relocate  <- the opacity / scale update of 3DGS-MCMC's relocate_gs and add_new_gs
+ *                       (scene/gaussian_model.py: _update_params with the compute_relocation CUDA kernel) and its
+ *                       replace_tensors_to_optimizer; gsplat strategy/ops.py relocate / sample_add
+ * For the n pairs (src[j], dst[j]) (DEVICE int64 [n]) with ratio[j] (DEVICE int32 [n]: 1 + the number of times src[j]
+ * was drawn): the caller has already copied row src[j] to row dst[j] of every per-Gaussian tensor.  With x the raw
+ * opacity of row dst[j], o = sigmoid(x), N = min(ratio[j], 51):
+ *   o' = 1 - (1 - o)^(1/N),
+ *   D  = sum_{i=1..N} sum_{k=0..i-1} C(i-1,k) (-1)^k o'^(k+1) / sqrt(k+1),
+ *   opacity <- logit(clamp(o', min_opacity, 1 - 2^-23)),   scaling[k] <- log((o / D) exp(scaling[k]))
+ * written to rows dst[j] AND src[j] of opacity [rows,1] and scaling [rows,3] (raw, in place).  Everything is evaluated
+ * in double (the published kernels use float32, where the alternating sum cancels badly at large N); D uses the
+ * unclamped o'.  N = 1 keeps the raw values unless the clamp applies.  1 - (1 - o')^N = o before the clamp.
+ * zero: HOST array of n_zero <= 32 descriptors; descriptor t's dst [rows, row_floats] float32 is zeroed at row dst[j],
+ * and also at row src[j] when zero_new != 0 (the twelve Adam moments; the densification accumulators pass 0).  Its
+ * src field is not read.
+ * Rows dst[.] must be distinct and disjoint from rows src[.] (the same src may repeat): thread j reads only row dst[j].
+ * One launch, no host synchronisation.  n == 0 does nothing.
+ * S3G_ERR_ARG before any launch: n < 0; n_zero outside 0..32 or a NULL descriptor array with n_zero > 0; with n > 0, a
+ * NULL pointer, a descriptor with a NULL dst or row_floats <= 0, or min_opacity outside (0, 1).
+ *
+ * s3g_mcmc_noise  <- the noise block after optimizer.step() in 3DGS-MCMC's train.py (build_scaling_rotation,
+ *                    op_sigmoid, torch.bmm); gsplat MCMCStrategy inject_noise_to_position
+ * xyz DEVICE float [P,3] (in place), the raw scaling [P,3], rotation [P,4] (w,x,y,z, not normalised) and opacity [P],
+ * eps [P,3] (standard normal):
+ *   gate = 1 / (1 + exp(-100 ((1 - sigmoid(opacity)) - 0.995))),  Sigma = R(q) diag(exp(scaling)^2) R(q)^T,
+ *   xyz += step * gate * Sigma eps,   step = xyz_lr * noise_lr.
+ * One elementwise launch: 56 bytes read and 12 written per Gaussian.  P == 0 does nothing.
+ * S3G_ERR_ARG before any launch: P < 0, a NULL pointer, P > INT_MAX / 4. */
+int s3g_mcmc_relocate(int n, const int64_t* src, const int64_t* dst, const int32_t* ratio, float min_opacity,
+                      float* opacity, float* scaling, int n_zero, const s3g_row_tensor* zero, void* stream);
+int s3g_mcmc_noise(int P, float* xyz, const float* scaling, const float* rotation, const float* opacity,
+                   const float* eps, float step, void* stream);
+
 /* ---- initialisation -------------------------------------------------------------------------
  * s3g_knn_mean_dist2  <- simple_knn._C.distCUDA2 (SimpleKNN::knn)   submodules/simple-knn/simple_knn.cu:185-221,
  *                        called at scene/gaussian_model.py:153 to initialise the scales

@@ -96,6 +96,9 @@ SIGNATURES = {
     "s3g_peer_all_gather": (_I, [_I, _I, _V, _I64, _V]),
     "s3g_peer_nvls_all_reduce": (_I, [_I, _I, _V, _I64, _V]),
     "s3g_gather_rows": (_I, [_I, _V, _I64, _I64, _V, _V]),
+    # MCMC densification; s3g_mcmc_relocate takes a host array of RowTensor (below)
+    "s3g_mcmc_relocate": (_I, [_I, _V, _V, _V, _F, _V, _V, _I, _V, _V]),
+    "s3g_mcmc_noise": (_I, [_I, _V, _V, _V, _V, _V, _F, _V]),
     "s3g_plane_reg_workspace_bytes": (_SZ, [_I, _V]),
     "s3g_plane_reg_forward": (_I, [_I, _V, _V, _V, _V]),
     "s3g_plane_reg_backward": (_I, [_I, _V, _V, _V]),

@@ -33,6 +33,16 @@ Not in the reference either: the absolute screen-space gradient statistic (AbsGS
 which prune and ``spatial_sort`` carry and densify resets like ``xyz_gradient_accum``; ``densify(..., max_grad_abs=T)``
 then selects clones and splits on ``||xyz_gradient_accum_abs / denom|| >= T``.  It is not saved: ``capture()`` keeps the
 reference's 14-tuple and ``restore()`` starts the accumulator from zero.
+
+Not in the reference either: 3DGS-MCMC's densification (Kheradmand et al. 2024; gsplat ``MCMCStrategy``; mcmc.py), an
+alternative to densify / prune with the same names as 3DGS-MCMC.  ``relocate_gs()`` moves every Gaussian with opacity
+<= 0.005 onto an alive one drawn by opacity, ``add_new_gs(cap_max)`` grows the model by at most 5 % up to ``cap_max``,
+and ``inject_noise(xyz_lr)`` adds covariance-shaped position noise to low-opacity Gaussians after each optimizer step.
+Each row copy is the one ``s3g_gather_rows`` launch of densify, followed by one ``s3g_mcmc_relocate`` launch that sets
+the drawn rows' and their copies' opacity and scales, zeroes the Adam moments of both and zeroes the copies'
+accumulators.  Zeroing the copies' moments differs from the published code, which zeroes only the drawn rows' and lets a
+relocated row keep the moments of the Gaussian it replaced.  ``filter_3D`` and ``_deformation_table`` follow the copies.
+``capture()`` keeps the reference's 14-tuple: the budget is the loop's to keep.
 """
 from __future__ import annotations
 
@@ -501,6 +511,65 @@ class GaussianModel:
                 big_points_ws = self.get_scaling.max(dim=1).values > 0.1 * extent
                 prune_mask = torch.logical_or(torch.logical_or(prune_mask, big_points_vs), big_points_ws)
             self.prune_points(prune_mask)
+
+    # ---- 3DGS-MCMC densification (mcmc.py) ---------------------------------------------------------------------------
+    def _mcmc_relocate_rows(self, src, dst, min_opacity):
+        """After _rebuild copied row src[j] to row dst[j]: both get the relocated opacity and scales, the Adam moments
+        of both and the accumulators of dst[j] become zero.  One launch."""
+        from .mcmc import relocate
+        counts = torch.bincount(src, minlength=self._xyz.shape[0])
+        zero = []
+        if self.optimizer is not None:
+            for name in PARAM_GROUPS:
+                st = self.optimizer.state.get(getattr(self, _ATTR[name]), None)
+                if st:
+                    zero += [(st["exp_avg"], True), (st["exp_avg_sq"], True)]
+        zero += [(t, False) for t in (self.xyz_gradient_accum, self.xyz_gradient_accum_abs, self.denom,
+                                      self._deformation_accum, self.max_radii2D)]
+        relocate(self._opacity.data, self._scaling.data, src, dst, counts[src] + 1, min_opacity, zero)
+
+    def relocate_gs(self, min_opacity=0.005, generator=None):
+        """3DGS-MCMC's relocate_gs: every dead Gaussian (opacity <= min_opacity) becomes a copy of an alive one drawn
+        with probability proportional to its opacity (with replacement); the drawn Gaussian and its copies share the
+        relocated opacity and scales.  P is unchanged.  Unlike the published code, the copies' Adam moments are zeroed
+        too, not only the drawn rows'."""
+        with torch.no_grad():
+            o = self.get_opacity.squeeze(1)
+            dead = o <= min_opacity
+            dead_idx = torch.nonzero(dead, as_tuple=False).squeeze(1)
+            alive_idx = torch.nonzero(~dead, as_tuple=False).squeeze(1)
+            if dead_idx.numel() == 0 or alive_idx.numel() == 0:
+                return
+            drawn = alive_idx[torch.multinomial(o[alive_idx], dead_idx.numel(), replacement=True, generator=generator)]
+            idx = torch.arange(o.shape[0], device=o.device)
+            idx[dead_idx] = drawn
+            self._rebuild(idx, o.shape[0], keep_accumulators=True)
+            self._mcmc_relocate_rows(drawn, dead_idx, min_opacity)
+
+    def add_new_gs(self, cap_max, generator=None, min_opacity=0.005):
+        """3DGS-MCMC's add_new_gs: grow by min(cap_max, int(1.05 P)) - P Gaussians (none once P >= cap_max), each a
+        copy of a row drawn with probability proportional to its opacity; drawn rows and copies share the relocated
+        opacity and scales (its opacity clamped below at min_opacity).  Returns the number added."""
+        P = self._xyz.shape[0]
+        n = max(0, min(int(cap_max), int(1.05 * P)) - P)
+        if n == 0:
+            return 0
+        with torch.no_grad():
+            o = self.get_opacity.squeeze(1)
+            drawn = torch.multinomial(o, n, replacement=True, generator=generator)
+            self._rebuild(torch.cat((torch.arange(P, device=o.device), drawn)), P, keep_accumulators=True)
+            self._mcmc_relocate_rows(drawn, torch.arange(P, P + n, device=o.device), min_opacity)
+        return n
+
+    def inject_noise(self, xyz_lr, noise_lr=5e5, generator=None):
+        """3DGS-MCMC's position noise, after optimizer.step(): xyz += xyz_lr * noise_lr * gate(o) * Sigma eps with
+        Sigma = R diag(s^2) R^T of the canonical parameters (not the 3-D-filtered scales), eps ~ N(0, I) [P,3] from
+        torch.randn with `generator`, gate = 1 / (1 + exp(-100 ((1 - o) - 0.995))).  One launch besides the randn."""
+        from .mcmc import inject_noise
+        with torch.no_grad():
+            eps = torch.randn(self._xyz.shape, device=self._xyz.device, generator=generator)
+            inject_noise(self._xyz.data, self._scaling.data, self._rotation.data, self._opacity.data,
+                         float(xyz_lr) * float(noise_lr), eps)
 
     def replace_tensor_to_optimizer(self, tensor, name):
         """gaussian_model.py:397-409: new parameter values, Adam moments reset to zero, step kept."""
