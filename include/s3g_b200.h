@@ -176,7 +176,8 @@ typedef struct s3g_peer_sink {
  * rasterize_points.cu:154-163).  dL_dconic [P,4] and dL_ddepth [P] are the
  * reference's internal intermediates; pass NULL unless you want them exported
  * (parity tests do).  dL_dmean2D is [P,3] with z untouched = 0
- * (backward.cu:578-579).
+ * (backward.cu:578-579).  dL_drot [P,4] must be 16-byte aligned (S3G_ERR_ARG
+ * before any launch otherwise; not read with a peer sink).
  * Optional extras:
  *   dL_dpix_aux, dL_dcolor_aux: both or neither, after a forward with colors_aux: `dL_dpix_aux` [3,H,W] ->
  *     `dL_dcolor_aux` [P,3]; the geometry gradients are then those of the SUM of both images' losses;

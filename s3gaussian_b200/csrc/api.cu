@@ -625,6 +625,8 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
     if (!sink && (!b.dL_dmean2D || !b.dL_dopacity || !b.dL_dcolor || !b.dL_dmean3D || !b.dL_dcov3D || !b.dL_dscale ||
                   !b.dL_drot))
         return fail(S3G_ERR_ARG, "backward: null gradient output");
+    if (!sink && (reinterpret_cast<uintptr_t>(b.dL_drot) & 15))
+        return fail(S3G_ERR_ARG, "backward: dL_drot must be 16-byte aligned (its [P,4] rows are stored 16 bytes at a time)");
     if (sink) {
         if (!b.dL_dmean2D || !b.dL_dcolor) return fail(S3G_ERR_ARG, "backward_dp: dL_dmean2D / dL_dcolor stay local and must be given");
         if (s.cov3D_precomp) return fail(S3G_ERR_ARG, "backward_dp: precomputed 3-D covariances are not exchanged");

@@ -509,6 +509,12 @@ class _RasterizeGaussians(torch.autograd.Function):
                 raise NotImplementedError("FusedGradExchange: an antialiased forward's gradients are not exchanged")
             _GRAD_SINK.note_backward()
             bwd.sink = C.pointer(peer)
+        # the kernel stores dL_drot 16 bytes per row: a sink's view off a 16-byte boundary (a flat bucket holding the
+        # tensors back to back, as bench.py lays it out for N > 1) receives the rows through an aligned tensor
+        rot_out = grad_rotations
+        if not bwd.sink and P > 0 and grad_rotations.data_ptr() % 16:
+            rot_out = torch.empty_like(grad_rotations)
+            bwd.dL_drot = _ptr(rot_out)
         grad_abs = None
         call = lambda: _backward_call(lib, scene, bwd, dev, P, H, W, opa)
         if absgrad:
@@ -524,6 +530,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                         raise ex
                 else:
                     call()
+                if rot_out is not grad_rotations:
+                    grad_rotations.copy_(rot_out)
             if any(cam_needs):
                 cam_grads = _camera_backward_call(lib, scene, bwd, dev, P, ctx.cam_shapes, cam_needs)
 

@@ -114,6 +114,27 @@ def test_rasterizer_extras_that_do_not_combine_are_rejected(built_lib):
     assert b"peer sink and the aux gradients do not combine" in lib.s3g_last_error()
 
 
+def test_backward_rejects_an_unaligned_rotation_gradient(built_lib):
+    """dL_drot is stored 16 bytes per row: an output off a 16-byte boundary is S3G_ERR_ARG before any launch, in the
+    plain, deterministic and absgrad backwards (the Python glue hands such a sink view an aligned tensor instead)."""
+    from s3gaussian_b200 import _lib
+    lib = built_lib
+    fake = 1 << 20    # never dereferenced: every call below fails validation first
+    scene = _lib.RasterScene(P=4, background=fake, width=16, height=16, means3D=fake, colors_precomp=fake,
+                             opacities=fake, scales=fake, scale_modifier=1.0, rotations=fake, viewmatrix=fake,
+                             projmatrix=fake, tan_fovx=1.0, tan_fovy=1.0)
+    for off in (4, 8, 12):
+        bwd = _lib.RasterBackwardArgs(R=5, geom_buffer=fake, binning_buffer=fake, image_buffer=fake, dL_dpix=fake,
+                                      dL_dpix_depth=fake, dL_dmean2D=fake, dL_dopacity=fake, dL_dcolor=fake,
+                                      dL_dmean3D=fake, dL_dcov3D=fake, dL_dscale=fake, dL_drot=fake + off)
+        for call in (lambda: lib.s3g_rasterize_backward(C.byref(scene), C.byref(bwd), None),
+                     lambda: lib.s3g_rasterize_backward_deterministic(C.byref(scene), C.byref(bwd), fake, None),
+                     lambda: lib.s3g_rasterize_backward_absgrad(C.byref(scene), C.byref(bwd), None, fake, 0, None,
+                                                                None)):
+            assert call() == -1, off
+            assert b"dL_drot must be 16-byte aligned" in lib.s3g_last_error(), (off, lib.s3g_last_error())
+
+
 def test_rasterizer_python_api_mirrors_reference_validation():
     from s3gaussian_b200 import diff_gaussian_rasterization as dgr
     assert dgr.GaussianRasterizationSettings._fields == (
