@@ -2,7 +2,7 @@
 train.py (scene_reconstruction, train.py:330-530) with every heavy step running through libs3g_b200.so.
 
     python examples/train_loop.py [--points 200000] [--iters 300] [--fine] [--filter-3d] [--densify-until N]
-                                 [--absgrad-threshold T | --mcmc-cap N]
+                                 [--absgrad-threshold T | --mcmc-cap N] [--sparse-adam]
 
 Synthetic data (there is no dataset reader here): a random cloud initialised through create_from_pcd
 (3-NN scales), targets rendered from a perturbed copy of it.  Needs a CUDA device (sm_90a).
@@ -38,6 +38,9 @@ def main():
     ap.add_argument("--mcmc-cap", type=int, default=0,
                     help="3DGS-MCMC densification up to this many Gaussians instead of densify / prune: relocation, "
                          "5 %% growth per interval, position noise and the opacity / scale regularisers (0: off)")
+    ap.add_argument("--sparse-adam", action="store_true",
+                    help="selective Adam: update only the Gaussians the step's view sees (radii > 0), as upstream "
+                         "3DGS --optimizer_type sparse_adam and gsplat SelectiveAdam")
     a = ap.parse_args()
     if a.mcmc_cap and a.absgrad_threshold > 0:
         ap.error("--mcmc-cap replaces densify / prune, so --absgrad-threshold has nothing to select")
@@ -116,7 +119,10 @@ def main():
                     gaussians.compute_3D_filter(cams)     # Mip-Splatting: after every densify and prune
             elif a.filter_3d and a.densify_until and it > a.densify_until and it % 100 == 0 and it < a.iters - 100:
                 gaussians.compute_3D_filter(cams)         # then every 100 iterations, except near the end
-        gaussians.optimizer.step()                                               # one launch over all groups
+        if a.sparse_adam:       # after densify / prune the per-Gaussian tensors have no gradient: dense groups only
+            gaussians.optimizer.step(visibility=out["radii"] > 0)
+        else:
+            gaussians.optimizer.step()                                           # one launch over all groups
         gaussians.optimizer.zero_grad(set_to_none=True)
         if a.mcmc_cap:
             gaussians.inject_noise(xyz_lr)

@@ -647,6 +647,8 @@ int s3g_sort_pairs_u32(int64_t n, uint32_t* keys_in, uint32_t* vals_in,
  *
  * s3g_adam_step       <- torch.optim.Adam(l, lr=0.0, eps=1e-15).step()   scene/gaussian_model.py:189, train.py:520-522
  *                        (torch/optim/adam.py _multi_tensor_adam: no weight decay, no amsgrad)
+ * s3g_adam_step_selective <- the same step restricted to the visible rows of the per-Gaussian tensors (not in the
+ *                        reference)
  * s3g_densify_stats   <- max_radii2D update + add_densification_stats    train.py:489-491, scene/gaussian_model.py:693-695
  * s3g_image_loss_*    <- l1_loss + ssim + compute_depth("l2")            utils/loss_utils.py:20-96, train.py:395-419
  */
@@ -663,6 +665,19 @@ typedef struct s3g_adam_tensor {
 /* `tensors` is a HOST array of n descriptors (device pointers inside).  One kernel launch per
  * 40 tensors.  Tensors with numel == 0 are skipped. */
 int s3g_adam_step(int n, const s3g_adam_tensor* tensors, double beta1, double beta2, double eps, void* stream);
+
+/* Selective Adam (upstream 3DGS --optimizer_type sparse_adam, Taming 3DGS, gsplat SelectiveAdam): s3g_adam_step in which
+ * the per-Gaussian tensors update only the rows the step's views see.  row_width: HOST int32[n].  row_width[i] == 0
+ * marks a dense tensor (the s3g_adam_step update); row_width[i] > 0 a masked one of `rows` rows of row_width[i] floats
+ * (numel == rows * row_width[i], fewer than 2^31 elements).  visible: DEVICE uint8[rows] (a torch bool tensor's
+ * storage).  A masked row with visible[r] != 0 gets exactly the s3g_adam_step update; one with visible[r] == 0 keeps
+ * its param, exp_avg and exp_avg_sq bit for bit and its grad is not read.  `step` is the tensor's global counter, as
+ * in s3g_adam_step, so an all-visible mask gives s3g_adam_step's bits.  One launch per 40 tensors, dense and masked
+ * together; no host synchronisation.  S3G_ERR_ARG before any launch: n < 0, a NULL table, rows < 0, row_width < 0,
+ * numel < 0 or != rows * row_width, and, for a tensor with numel > 0, a NULL pointer, step < 1, or a NULL visible
+ * with row_width > 0. */
+int s3g_adam_step_selective(int n, const s3g_adam_tensor* tensors, const int32_t* row_width, int64_t rows,
+                            const uint8_t* visible, double beta1, double beta2, double eps, void* stream);
 
 /* radii i32[P] (max over the step's views), viewspace_grad f32[P,3] (summed over the views);
  * for radii > 0: max_radii2D = max(max_radii2D, radii); xyz_gradient_accum += |grad[:2]|; denom += 1. */

@@ -84,6 +84,8 @@ SIGNATURES = {
     "s3g_sort_pairs_u32": (_I, [_I64, _V, _V, _V, _V, _I, _I, _V, _V]),
     # training-step kernels; s3g_adam_step takes a host array of AdamTensor (below)
     "s3g_adam_step": (_I, [_I, _V, _D, _D, _D, _V]),
+    # and the selective step: tensors, row_width (HOST int32[n]), rows, visible (DEVICE uint8[rows])
+    "s3g_adam_step_selective": (_I, [_I, _V, _V, _I64, _V, _D, _D, _D, _V]),
     "s3g_densify_stats": (_I, [_I, _V, _V, _V, _V, _V, _V]),
     "s3g_densify_stats_abs": (_I, [_I, _V, _V, _V, _V, _V, _V, _V, _V]),
     "s3g_image_loss_workspace_bytes": (_SZ, [_I, _I, _I, _I]),

@@ -55,7 +55,63 @@ int s3g_adam_step(int n, const s3g_adam_tensor* tensors, double beta1, double be
     return S3G_OK;
 }
 
-int s3g_densify_stats(int P, const float* viewspace_grad, const int* radii, float* xyz_gradient_accum,
+int s3g_adam_step_selective(int n, const s3g_adam_tensor* tensors, const int32_t* row_width, int64_t rows,
+                            const uint8_t* visible, double beta1, double beta2, double eps, void* stream_) {
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (n < 0 || (n > 0 && (!tensors || !row_width))) return fail(S3G_ERR_ARG, "adam_step_selective: bad tensor table");
+    if (rows < 0) return fail(S3G_ERR_ARG, "adam_step_selective: rows < 0");
+    // every argument is checked before the first launch, so an error leaves every tensor as it was
+    long long total_blocks = 0;
+    for (int i = 0; i < n; ++i) {
+        const s3g_adam_tensor& t = tensors[i];
+        const int w = row_width[i];
+        if (w < 0) return fail(S3G_ERR_ARG, "adam_step_selective: row_width < 0");
+        if (t.numel < 0) return fail(S3G_ERR_ARG, "adam_step_selective: negative numel");
+        if (w > 0 && (t.numel % w != 0 || t.numel / w != rows))
+            return fail(S3G_ERR_ARG, "adam_step_selective: a masked tensor needs numel == rows * row_width");
+        if (t.numel == 0) continue;
+        if (!t.param || !t.grad || !t.exp_avg || !t.exp_avg_sq || t.step < 1)
+            return fail(S3G_ERR_ARG, "adam_step_selective: null pointer or step < 1");
+        if (w > 0 && !visible) return fail(S3G_ERR_ARG, "adam_step_selective: null visible");
+        if (w > 0 && t.numel > 0x7fffffffLL)
+            return fail(S3G_ERR_ARG, "adam_step_selective: a masked tensor must have fewer than 2^31 elements");
+        total_blocks += (t.numel + ADAM_CHUNK - 1) / ADAM_CHUNK;
+        if (total_blocks > 0x7fffffffLL) return fail(S3G_ERR_ARG, "adam_step_selective: tensors too large");
+    }
+    AdamSelectiveArgs a;
+    a.w1 = (float)(1.0 - beta1);
+    a.beta2 = (float)beta2;
+    a.omb2 = (float)(1.0 - beta2);
+    a.eps = (float)eps;
+    a.visible = visible;
+    int i = 0;
+    while (i < n) {
+        a.count = 0;
+        int blocks = 0;
+        for (; i < n && a.count < ADAM_MAX_TENSORS; ++i) {
+            const s3g_adam_tensor& t = tensors[i];
+            if (t.numel == 0) continue;
+            AdamTensor& d = a.t[a.count];
+            d.p = t.param; d.g = t.grad; d.m = t.exp_avg; d.v = t.exp_avg_sq; d.n = t.numel;
+            const double bc1 = 1.0 - std::pow(beta1, (double)t.step);
+            const double bc2 = 1.0 - std::pow(beta2, (double)t.step);
+            d.step_size = (float)(t.lr / bc1);
+            d.bc2_sqrt = (float)std::sqrt(bc2);
+            a.row_width[a.count] = (unsigned)row_width[i];
+            a.block_start[a.count] = blocks;
+            blocks += (int)((t.numel + ADAM_CHUNK - 1) / ADAM_CHUNK);
+            ++a.count;
+        }
+        a.block_start[a.count] = blocks;
+        if (blocks > 0) {
+            adam_selective_kernel<<<blocks, ADAM_THREADS, 0, stream>>>(a);
+            S3G_CUDA(cudaGetLastError(), "adam_step_selective launch");
+        }
+    }
+    return S3G_OK;
+}
+
+int s3g_densify_stats(int P,const float* viewspace_grad, const int* radii, float* xyz_gradient_accum,
                       float* denom, float* max_radii2D, void* stream_) {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     if (P < 0) return fail(S3G_ERR_ARG, "densify_stats: P < 0");

@@ -96,6 +96,113 @@ __global__ void __launch_bounds__(ADAM_THREADS) adam_multi_tensor_kernel(const _
 }
 
 // ---------------------------------------------------------------------------------------------
+// Selective Adam (upstream 3DGS --optimizer_type sparse_adam, Taming 3DGS, gsplat SelectiveAdam): the tensors with
+// row_width[i] > 0 hold `rows` rows of row_width floats, and only the rows with visible[r] != 0 are updated; every
+// other row keeps its parameter and both moments bit for bit, and its gradient is never read.  Tensors with
+// row_width 0 get the dense update in the same launch.  Every updated element gets adam_multi_tensor_kernel's
+// arithmetic and roundings (adam_update_exact), so an all-visible mask, and a dense tensor under any mask, equal the
+// dense step bit for bit.
+// Same chunking as the dense kernel, one float4 per thread at a time.  In a masked tensor each thread looks up the
+// rows its float4 spans (at most 4; the mask is 1 byte per row and stays in L1 / L2) and skips a float4 with no
+// visible row without touching p, g, m or v, so an invisible row costs no parameter, gradient or moment traffic
+// beyond the sectors it shares with a visible one.  A float4 whose rows are all visible takes the vector path; one
+// that mixes takes predicated scalar accesses, as does every element of a tensor that is not 16-byte aligned.
+// ---------------------------------------------------------------------------------------------
+struct AdamSelectiveArgs {
+    AdamTensor t[ADAM_MAX_TENSORS];
+    unsigned row_width[ADAM_MAX_TENSORS];     // 0: dense; masked tensors have n < 2^32
+    int block_start[ADAM_MAX_TENSORS + 1];
+    int count;
+    float w1, beta2, omb2, eps;
+    const unsigned char* visible;             // [rows]
+};
+
+// adam_update with every rounding spelled out.  ptxas contracts adam_update's last line, p - step_size * q, into one
+// FFMA in some places of adam_multi_tensor_kernel and not in others: as compiled for sm_90a, the scalar path and the
+// .w lane of the float4 path round once (fused), the .x, .y and .z lanes round the product and then the difference.
+// Naming the rounding per element lets the selective kernel give every element the dense kernel's bits, whatever
+// ptxas would choose here.
+__device__ __forceinline__ void adam_update_exact(float& p, float g, float& m, float& v, float w1, float b2, float omb2,
+                                                  float eps, float step_size, float bc2_sqrt, bool fused) {
+    m = fmaf(w1, __fsub_rn(g, m), m);
+    v = fmaf(__fmul_rn(omb2, g), g, __fmul_rn(v, b2));
+    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), eps);
+    const float q = __fdiv_rn(m, denom);
+    p = fused ? fmaf(-step_size, q, p) : __fsub_rn(p, __fmul_rn(step_size, q));
+}
+
+__global__ void __launch_bounds__(ADAM_THREADS) adam_selective_kernel(const __grid_constant__ AdamSelectiveArgs a) {
+    int lo = 0, hi = a.count;
+    const int b = blockIdx.x;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (a.block_start[mid] <= b) lo = mid; else hi = mid;
+    }
+    const AdamTensor& t = a.t[lo];
+    const unsigned w = a.row_width[lo];
+    const unsigned char* __restrict__ vis = a.visible;
+    const long long base = (long long)(b - a.block_start[lo]) * ADAM_CHUNK;
+    const long long end = (base + ADAM_CHUNK < t.n) ? base + ADAM_CHUNK : t.n;
+    const float ss = t.step_size, bc = t.bc2_sqrt;
+    const bool aligned = ((((uintptr_t)t.p) | ((uintptr_t)t.g) | ((uintptr_t)t.m) | ((uintptr_t)t.v)) & 15) == 0;
+    const bool dense_vec = aligned && base + ADAM_CHUNK <= t.n;     // the dense kernel's float4 path takes this chunk
+    if (aligned) {
+        // the mask bytes of all four float4s first, so their latency is paid once and not before each float4
+        unsigned any = 0xfu, all = 0xfu;
+        if (w != 0) {
+            any = all = 0u;
+#pragma unroll
+            for (int j = 0; j < ADAM_VEC_PER_THREAD; ++j) {
+                const long long i = base + (long long)(j * ADAM_THREADS + threadIdx.x) * 4;
+                if (i >= end) break;
+                const long long last = i + 3 < end ? i + 3 : end - 1;
+                bool a_ = false, b_ = true;
+                for (unsigned r = (unsigned)i / w, r1 = (unsigned)last / w; r <= r1; ++r) {
+                    const bool s = __ldg(vis + r) != 0;
+                    a_ |= s;
+                    b_ &= s;
+                }
+                any |= (unsigned)a_ << j;
+                all |= (unsigned)b_ << j;
+            }
+        }
+        for (int j = 0; j < ADAM_VEC_PER_THREAD; ++j) {
+            const long long i = base + (long long)(j * ADAM_THREADS + threadIdx.x) * 4;
+            if (i >= end) break;
+            const long long last = i + 3 < end ? i + 3 : end - 1;
+            if (!((any >> j) & 1u)) continue;
+            if (((all >> j) & 1u) && last == i + 3) {
+                const float4 G = __ldcs(reinterpret_cast<const float4*>(t.g + i));
+                float4 P = *reinterpret_cast<const float4*>(t.p + i);
+                float4 M = *reinterpret_cast<const float4*>(t.m + i);
+                float4 V = *reinterpret_cast<const float4*>(t.v + i);
+                adam_update_exact(P.x, G.x, M.x, V.x, a.w1, a.beta2, a.omb2, a.eps, ss, bc, !dense_vec);
+                adam_update_exact(P.y, G.y, M.y, V.y, a.w1, a.beta2, a.omb2, a.eps, ss, bc, !dense_vec);
+                adam_update_exact(P.z, G.z, M.z, V.z, a.w1, a.beta2, a.omb2, a.eps, ss, bc, !dense_vec);
+                adam_update_exact(P.w, G.w, M.w, V.w, a.w1, a.beta2, a.omb2, a.eps, ss, bc, true);
+                *reinterpret_cast<float4*>(t.p + i) = P;
+                *reinterpret_cast<float4*>(t.m + i) = M;
+                *reinterpret_cast<float4*>(t.v + i) = V;
+                continue;
+            }
+            for (long long e = i; e <= last; ++e) {
+                if (w != 0 && !__ldg(vis + (unsigned)e / w)) continue;
+                float p = t.p[e], m = t.m[e], v = t.v[e];
+                adam_update_exact(p, t.g[e], m, v, a.w1, a.beta2, a.omb2, a.eps, ss, bc, !dense_vec || (e & 3) == 3);
+                t.p[e] = p; t.m[e] = m; t.v[e] = v;
+            }
+        }
+    } else {
+        for (long long e = base + threadIdx.x; e < end; e += ADAM_THREADS) {
+            if (w != 0 && !__ldg(vis + (unsigned)e / w)) continue;
+            float p = t.p[e], m = t.m[e], v = t.v[e];
+            adam_update_exact(p, t.g[e], m, v, a.w1, a.beta2, a.omb2, a.eps, ss, bc, true);
+            t.p[e] = p; t.m[e] = m; t.v[e] = v;
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Densification statistics (train.py:489-491 + GaussianModel.add_densification_stats):
 //   vis = radii > 0 ; max_radii2D[vis] = max(max_radii2D[vis], radii[vis]) ;
 //   xyz_gradient_accum[vis] += |viewspace_grad[vis, :2]| ; denom[vis] += 1

@@ -7,7 +7,9 @@ Same attribute and method names as the reference so ``train.py``-style loops rea
 ``prune_points``, ``reset_opacity``, ``compute_regulation`` ...).  What differs is how the work runs:
 
 * the optimizer is ``FusedAdam`` (one launch per step, optim.py) with the reference's eight groups
-  and learning rates (scene/gaussian_model.py:176-189);
+  and learning rates (scene/gaussian_model.py:176-189).  Its per-Gaussian groups are the six of ``PARAM_GROUPS``, so
+  ``optimizer.step(visibility=radii > 0)`` is selective Adam (only the rows the step's views see are updated);
+  ``optimizer.step()`` is the reference's dense step;
 * densify / prune rebuild the six parameters, their twelve Adam moments and the four per-Gaussian
   accumulators with ONE row-gather launch per operation (``s3g_gather_rows``) instead of boolean
   indexing + ``torch.cat`` per tensor (gaussian_model.py:411-470); the small mask / index arithmetic
@@ -279,7 +281,7 @@ class GaussianModel:
                    {"params": [self._opacity], "lr": training_args.opacity_lr, "name": "opacity"},
                    {"params": [self._scaling], "lr": training_args.scaling_lr, "name": "scaling"},
                    {"params": [self._rotation], "lr": training_args.rotation_lr, "name": "rotation"}]
-        self.optimizer = FusedAdam(groups, lr=0.0, eps=1e-15)
+        self.optimizer = FusedAdam(groups, lr=0.0, eps=1e-15, selective_groups=PARAM_GROUPS)
         self.xyz_scheduler_args = get_expon_lr_func(training_args.position_lr_init * s, training_args.position_lr_final * s,
                                                     lr_delay_mult=training_args.position_lr_delay_mult,
                                                     max_steps=training_args.position_lr_max_steps)

@@ -24,13 +24,25 @@ from . import _lib
 
 
 class FusedAdam(torch.optim.Optimizer):
+    """``selective_groups``: names of the param groups whose tensors hold one row per Gaussian (``[P, ...]``,
+    contiguous).  ``step(visibility=v)`` with ``v`` a bool CUDA tensor ``[P]`` (``radii > 0`` of the step's render, or
+    the union over its views) is then selective Adam (upstream 3DGS ``sparse_adam``, gsplat ``SelectiveAdam``): in
+    those groups only the rows with ``v[i]`` are updated and every other row keeps its parameter and both moments
+    bit for bit (its gradient is not read); the other groups get the dense update in the same launch.  The step
+    counter and the bias correction stay global, so an all-true ``v`` gives ``step()``'s bits.  A tensor without a
+    gradient is skipped as in ``step()``.  The names are a constructor argument, not a param-group key, so they
+    survive ``load_state_dict`` of a torch.optim.Adam checkpoint."""
+
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, *,
-                 maximize=False):
+                 maximize=False, selective_groups=()):
         if weight_decay != 0 or amsgrad or maximize:
             raise NotImplementedError("FusedAdam: weight_decay / amsgrad / maximize are not used by the "
                                       "reference (scene/gaussian_model.py:189) and not implemented")
         if lr < 0.0 or eps < 0.0 or not (0.0 <= betas[0] < 1.0) or not (0.0 <= betas[1] < 1.0):
             raise ValueError("FusedAdam: invalid lr / eps / betas")
+        if isinstance(selective_groups, str):
+            raise TypeError("FusedAdam: selective_groups is a collection of group names")
+        self.selective_groups = frozenset(selective_groups)
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=amsgrad,
                                       maximize=maximize))
 
@@ -42,49 +54,77 @@ class FusedAdam(torch.optim.Optimizer):
             st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
         return st
 
+    def _check_visibility(self, v):
+        if not isinstance(v, torch.Tensor) or v.dtype != torch.bool or v.dim() != 1 or not v.is_contiguous():
+            raise RuntimeError("FusedAdam.step: visibility must be a contiguous 1-D bool tensor")
+        if not any(g.get("name") in self.selective_groups for g in self.param_groups):
+            raise RuntimeError("FusedAdam.step: visibility given, but the optimizer has no per-Gaussian group "
+                               f"(selective_groups={sorted(self.selective_groups)})")
+
     @torch.no_grad()
-    def step(self, closure=None):
+    def step(self, closure=None, *, visibility=None):
         loss = None
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
-        lib = _lib.load()
-        by_key = {}     # (device index, betas, eps) -> descriptors; one launch per 40 tensors each
-        keep = []
+        v = visibility
+        if v is not None:
+            self._check_visibility(v)
+        # every check runs before any state changes or any launch
+        todo = []
         for group in self.param_groups:
-            b1, b2 = group["betas"]
+            masked = v is not None and group.get("name") in self.selective_groups
             for p in group["params"]:
                 if p.grad is None:
                     continue
+                if masked:
+                    if p.dim() == 0 or p.shape[0] != v.numel():
+                        raise RuntimeError(f"FusedAdam.step: group {group.get('name')!r} has {tuple(p.shape)} rows "
+                                           f"for a visibility of {v.numel()}")
+                    if p.device != v.device:
+                        raise RuntimeError("FusedAdam.step: visibility must be on the parameters' device")
                 if not p.is_cuda or p.dtype != torch.float32:
                     raise RuntimeError("FusedAdam: CUDA float32 parameters only (there is no CPU path)")
-                g = p.grad
-                if g.is_sparse:
+                if p.grad.is_sparse:
                     raise RuntimeError("FusedAdam does not support sparse gradients")
                 # the update is elementwise: any dense layout works as long as all four tensors share it
-                # (HexPlane planes are channels_last)
+                # (HexPlane planes are channels_last); masked rows must be contiguous
                 if p.is_contiguous():
                     fmt = torch.contiguous_format
-                elif p.dim() == 4 and p.is_contiguous(memory_format=torch.channels_last):
+                elif not masked and p.dim() == 4 and p.is_contiguous(memory_format=torch.channels_last):
                     fmt = torch.channels_last
                 else:
-                    raise RuntimeError("FusedAdam: parameters must be dense (contiguous or channels_last)")
-                if g.stride() != p.stride():
-                    g = g.contiguous(memory_format=fmt)
-                st = self._init_state(p)
-                for k in ("exp_avg", "exp_avg_sq"):
-                    if st[k].stride() != p.stride():
-                        st[k] = st[k].contiguous(memory_format=fmt)
-                st["step"] += 1
-                keep.append(g)
-                by_key.setdefault((p.device.index, float(b1), float(b2), float(group["eps"])), []).append(
-                    _lib.AdamTensor(p.data_ptr(), g.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr(),
-                                    p.numel(), float(group["lr"]), int(st["step"])))
-        for (dev, b1, b2, eps), descs in by_key.items():
+                    raise RuntimeError("FusedAdam: parameters must be dense (contiguous or channels_last)" +
+                                       ("; per-Gaussian ones contiguous" if masked else ""))
+                todo.append((group, p, fmt, p.numel() // p.shape[0] if masked and p.numel() else 0))
+        lib = _lib.load()
+        by_key = {}     # (device index, betas, eps) -> (descriptors, row widths); one launch per 40 tensors each
+        keep = []
+        for group, p, fmt, width in todo:
+            b1, b2 = group["betas"]
+            g = p.grad
+            if g.stride() != p.stride():
+                g = g.contiguous(memory_format=fmt)
+            st = self._init_state(p)
+            for k in ("exp_avg", "exp_avg_sq"):
+                if st[k].stride() != p.stride():
+                    st[k] = st[k].contiguous(memory_format=fmt)
+            st["step"] += 1
+            keep.append(g)
+            descs, widths = by_key.setdefault((p.device.index, float(b1), float(b2), float(group["eps"])), ([], []))
+            descs.append(_lib.AdamTensor(p.data_ptr(), g.data_ptr(), st["exp_avg"].data_ptr(),
+                                         st["exp_avg_sq"].data_ptr(), p.numel(), float(group["lr"]), int(st["step"])))
+            widths.append(width)
+        for (dev, b1, b2, eps), (descs, widths) in by_key.items():
             arr = (_lib.AdamTensor * len(descs))(*descs)
             with torch.cuda.device(dev):
                 stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-                _lib.check(lib.s3g_adam_step(len(descs), arr, b1, b2, eps, stream), "s3g_adam_step")
+                if v is None:
+                    _lib.check(lib.s3g_adam_step(len(descs), arr, b1, b2, eps, stream), "s3g_adam_step")
+                else:
+                    w = (C.c_int32 * len(widths))(*widths)
+                    _lib.check(lib.s3g_adam_step_selective(len(descs), arr, w, v.numel(), v.data_ptr(), b1, b2, eps,
+                                                           stream), "s3g_adam_step_selective")
         return loss
 
 
