@@ -442,9 +442,11 @@ int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f
     S3G_MARK(0, "depth_sort");
 
     // ---- depth digits of the LSD sort, over Gaussians --------------------
+    // The offsets are first written by the scan below, so until then their buffer is the sort's second key scratch
+    // and depth_key keeps every Gaussian's key (what s3g_state_field exports under that name).
     S3G_CUDA(radix_sort_pairs((uint32_t)P, geom.depth_key, geom.order_a, geom.key_b, geom.order_b,
                               nullptr, geom.order_a, 0, 32, geom.sort, stream, nullptr, /*hist_ready=*/false,
-                              /*prepared=*/true),
+                              /*prepared=*/true, /*keys_spare=*/geom.offsets),
              "depth sort");
     S3G_STAGE("depth sort");
 

@@ -72,12 +72,15 @@ __device__ __forceinline__ uint32_t block_excl_scan_256(uint32_t v, uint32_t* s_
 // n: item count known on the host, or the capacity when `n_dev` (device word with the true count, clamped to n)
 // is given.  prepared: the caller already zeroed the temp block (radix_sort_prepare, e.g. folded into a larger
 // memset).  hist_ready (implies prepared): a producer kernel already wrote the digit histograms
-// st.hist[pass][digit]; otherwise the driver runs sort_histogram_kernel.
+// st.hist[pass][digit]; otherwise the driver runs sort_histogram_kernel.  keys_spare: a second key scratch of n
+// items; the intermediate keys then alternate between keys_tmp and keys_spare and keys_in keeps the input keys
+// (without it the second pass writes its keys back into keys_in).
 cudaError_t radix_sort_prepare(const SortTemp& st, cudaStream_t stream);
 cudaError_t radix_sort_pairs(uint32_t n, uint32_t* keys_in, uint32_t* vals_in, uint32_t* keys_tmp,
                              uint32_t* vals_tmp, uint32_t* keys_final, uint32_t* vals_final, int begin_bit,
                              int end_bit, const SortTemp& st, cudaStream_t stream,
-                             const uint32_t* n_dev = nullptr, bool hist_ready = false, bool prepared = false);
+                             const uint32_t* n_dev = nullptr, bool hist_ready = false, bool prepared = false,
+                             uint32_t* keys_spare = nullptr);
 
 #ifdef S3G_RADIX_SORT_IMPL
 // ---- histogram of every digit of every pass in one read of the keys -------
@@ -259,7 +262,7 @@ cudaError_t radix_sort_pairs(uint32_t n, uint32_t* keys_in, uint32_t* vals_in,
                                     uint32_t* keys_tmp, uint32_t* vals_tmp, uint32_t* keys_final,
                                     uint32_t* vals_final, int begin_bit, int end_bit,
                                     const SortTemp& st, cudaStream_t stream, const uint32_t* n_dev,
-                                    bool hist_ready, bool prepared) {
+                                    bool hist_ready, bool prepared, uint32_t* keys_spare) {
     if (n == 0) return cudaSuccess;
     int bits = end_bit - begin_bit;
     int npass = (bits + RADIX_BITS - 1) / RADIX_BITS;
@@ -281,7 +284,9 @@ cudaError_t radix_sort_pairs(uint32_t n, uint32_t* keys_in, uint32_t* vals_in,
     uint32_t* src_v = vals_in;
     for (int p = 0; p < npass; ++p) {
         const bool last = (p == npass - 1);
-        uint32_t* dst_k = last ? keys_final : (src_k == keys_in ? keys_tmp : keys_in);
+        uint32_t* dst_k = last ? keys_final
+                          : keys_spare ? (p % 2 == 0 ? keys_tmp : keys_spare)
+                                       : (src_k == keys_in ? keys_tmp : keys_in);
         uint32_t* dst_v = last ? vals_final : (src_v == vals_in ? vals_tmp : vals_in);
         int shift = begin_bit + p * RADIX_BITS;
         int pb = end_bit - shift < RADIX_BITS ? end_bit - shift : RADIX_BITS;

@@ -363,15 +363,47 @@ def test_full_size_properties(ours):
         assert e < 5e-4, (k, e)
 
 
+def _sort_keys(kind, n, b0, b1, hi, g):
+    """int32 keys (bit patterns of u32) of one standalone-sort input"""
+    rand = lambda lo_, hi_: torch.randint(lo_, hi_, (n,), device=DEV, generator=g, dtype=torch.int64)
+    if kind == "random":
+        k = rand(0, hi)
+    elif kind == "equal":                 # one key: every block's digits are all equal
+        k = torch.full((n,), 0x5A3C_96E1, device=DEV, dtype=torch.int64)
+    elif kind == "sorted":
+        k = torch.sort(rand(0, hi)).values
+    elif kind == "reverse":
+        k = torch.sort(rand(0, hi), descending=True).values
+    elif kind == "top_digit":             # only the last pass's digit differs; the lower bits are one constant
+        top = b0 + 8 * ((b1 - b0 - 1) // 8)
+        k = (rand(0, 1 << (b1 - top)) << top) | (0x00C3_A5F0 & ((1 << top) - 1))
+    elif kind == "pad_value":             # the onesweep pads the last block with 0xFFFFFFFF: real keys equal to it
+        k = torch.where(rand(0, 2) == 0, torch.full((n,), 0xFFFF_FFFF, device=DEV, dtype=torch.int64),
+                        rand(0, 1 << 32))
+    else:
+        raise ValueError(kind)
+    return (k - ((k >> 31) << 32)).to(torch.int32)   # u32 bit pattern as int32
+
+
 def test_radix_sort_standalone(built_lib):
-    """the hand-written onesweep sort vs torch.sort(stable=True), incl. ragged sizes"""
+    """the hand-written onesweep sort vs torch.sort(stable=True): ragged sizes (n = 4096 k +- 1 around 1, 8, 9 and
+    16 blocks, past the 8-block look-back window), all keys equal, sorted and reversed input, keys that differ only in
+    the top digit, keys equal to the onesweep's padding value, one pass over bits [24, 32) and last digits 1 bit wide"""
     import ctypes as C
     from s3gaussian_b200 import _lib
     lib = built_lib
     g = torch.Generator(device=DEV).manual_seed(0)
-    for n, b0, b1, hi in [(1, 0, 32, 2**31), (33, 0, 8, 200), (4096, 0, 32, 2**31), (4097, 0, 14, 9600),
-                          (123_457, 3, 17, 2**20), (1_000_003, 0, 14, 9600), (2_000_000, 0, 32, 2**31)]:
-        keys = torch.randint(0, hi, (n,), device=DEV, generator=g, dtype=torch.int64).to(torch.int32)
+    for n, b0, b1, hi, kind in [
+            (1, 0, 32, 2**31, "random"), (33, 0, 8, 200, "random"), (4096, 0, 32, 2**31, "random"),
+            (4097, 0, 14, 9600, "random"), (123_457, 3, 17, 2**20, "random"), (1_000_003, 0, 14, 9600, "random"),
+            (2_000_000, 0, 32, 2**31, "random"),
+            (4095, 0, 32, 0, "equal"), (4097, 0, 32, 0, "pad_value"), (8 * 4096 - 1, 0, 32, 0, "pad_value"),
+            (8 * 4096 + 1, 0, 32, 0, "equal"), (9 * 4096 - 1, 0, 32, 2**32, "sorted"),
+            (9 * 4096 + 1, 0, 32, 2**32, "reverse"), (16 * 4096 - 1, 0, 17, 0, "top_digit"),
+            (16 * 4096 + 1, 0, 32, 0, "top_digit"), (9 * 4096 + 1, 24, 32, 0, "top_digit"),
+            (16 * 4096 + 1, 24, 32, 2**32, "random"), (8 * 4096 + 1, 0, 17, 1 << 17, "random"),
+            (9 * 4096 - 1, 3, 12, 2**32, "reverse"), (4095, 0, 9, 0, "equal")]:
+        keys = _sort_keys(kind, n, b0, b1, hi, g)
         vals = torch.arange(n, device=DEV, dtype=torch.int32)
         ko, vo = torch.empty_like(keys), torch.empty_like(vals)
         tmp = torch.empty(lib.s3g_sort_temp_bytes(n), dtype=torch.uint8, device=DEV)
