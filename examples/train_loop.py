@@ -2,7 +2,7 @@
 train.py (scene_reconstruction, train.py:330-530) with every heavy step running through libs3g_b200.so.
 
     python examples/train_loop.py [--points 200000] [--iters 300] [--fine] [--filter-3d] [--densify-until N]
-                                 [--absgrad-threshold T | --mcmc-cap N] [--sparse-adam]
+                                 [--absgrad-threshold T | --mcmc-cap N] [--sparse-adam] [--bilateral-grid]
 
 Synthetic data (there is no dataset reader here): a random cloud initialised through create_from_pcd
 (3-NN scales), targets rendered from a perturbed copy of it.  Needs a CUDA device (sm_90a).
@@ -41,6 +41,10 @@ def main():
     ap.add_argument("--sparse-adam", action="store_true",
                     help="selective Adam: update only the Gaussians the step's view sees (radii > 0), as upstream "
                          "3DGS --optimizer_type sparse_adam and gsplat SelectiveAdam")
+    ap.add_argument("--bilateral-grid", action="store_true",
+                    help="per-camera bilateral-grid colour correction (gsplat --use_bilateral_grid): every camera's "
+                         "targets get a fixed exposure difference, and each render is sliced through its camera's "
+                         "grid before the loss")
     a = ap.parse_args()
     if a.mcmc_cap and a.absgrad_threshold > 0:
         ap.error("--mcmc-cap replaces densify / prune, so --absgrad-threshold has nothing to select")
@@ -65,6 +69,20 @@ def main():
         for c in cams:
             out = render(c, gt, pipe, bg, stage="coarse")
             targets.append((out["render"].clone(), out["depth"].clone()))
+    bil_grids = bil_opt = None
+    if a.bilateral_grid:
+        from s3gaussian_b200.bilateral_grid import BilateralGrid
+        from s3gaussian_b200.optim import FusedAdam
+        # each camera's own exposure and white balance: a fixed per-channel gain and offset on its targets
+        g = torch.Generator().manual_seed(7)
+        for k, (img, dep) in enumerate(targets):
+            gain = (1.0 + 0.15 * torch.randn(3, 1, 1, generator=g)).to(dev)
+            offset = (0.03 * torch.randn(3, 1, 1, generator=g)).to(dev)
+            targets[k] = (img * gain + offset, dep)
+        bil_grids = BilateralGrid(len(cams)).to(dev)
+        # gsplat's schedule (its LinearLR and ExponentialLR chained, so their factors multiply): lr 2e-3, a linear
+        # warm-up from 0.01x over the first 1000 iterations and an exponential decay to 0.01x at the last iteration
+        bil_opt = FusedAdam([{"params": [bil_grids.grids], "lr": 2e-3, "name": "bilagrid"}], lr=2e-3, eps=1e-15)
     colours = (truth.features_dc[:, 0] * 0.28209479177387814 + 0.5).clamp(0, 1)
     pcd = SimpleNamespace(points=truth.xyz.numpy(), colors=colours.numpy())
 
@@ -92,8 +110,12 @@ def main():
         k = (it - 1) % len(cams)
         out = render(cams[k], gaussians, train_pipe, bg, stage=stage, return_dx=a.fine, render_feat=False)
         image, depth = out["render"], out["depth"]
+        if bil_grids is not None:
+            image = bil_grids.slice(image, k)
         l1, ssim_value, depth_l2 = losses.image_loss_terms(image, targets[k][0], depth, targets[k][1])
         loss = l1 + 0.5 * depth_l2 + 0.2 * (1.0 - ssim_value)                    # train.py:395-419
+        if bil_grids is not None:
+            loss = loss + 10.0 * bil_grids.tv_loss()
         if a.fine:
             loss = loss + 0.001 * out["dx"].abs().mean() + 0.001 * out["dshs"].abs().mean() + \
                 gaussians.compute_regulation(0.01, 0.0001, 0.0001)
@@ -124,6 +146,12 @@ def main():
         else:
             gaussians.optimizer.step()                                           # one launch over all groups
         gaussians.optimizer.zero_grad(set_to_none=True)
+        if bil_opt is not None:
+            warm = 0.01 + 0.99 * min((it - 1) / 1000.0, 1.0)
+            decay = 0.01 ** ((it - 1) / a.iters)
+            bil_opt.param_groups[0]["lr"] = 2e-3 * warm * decay
+            bil_opt.step()
+            bil_opt.zero_grad(set_to_none=True)
         if a.mcmc_cap:
             gaussians.inject_noise(xyz_lr)
         if it % 50 == 0:

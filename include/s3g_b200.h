@@ -737,6 +737,51 @@ size_t s3g_plane_reg_workspace_bytes(int n, const s3g_plane_desc* planes);
 int s3g_plane_reg_forward(int n, const s3g_plane_desc* planes, double* total, void* workspace, void* stream);
 int s3g_plane_reg_backward(int n, const s3g_plane_desc* planes, const float* gscale, void* stream);
 
+/* ---- bilateral-grid colour correction (Wang et al., SIGGRAPH 2024; gsplat lib_bilagrid) ----------------------------
+ * Not in the reference.  Each training image n gets a grid [12, L, GY, GX] of 3x4 affine colour transforms, indexed by
+ * pixel position and luminance; the render is corrected through it before the photometric loss, so per-camera
+ * exposure and white balance stop being explained by geometry.  grids: DEVICE float [N, 12, L, GY, GX], channel c is
+ * entry (c / 4, c % 4) of the matrix A.  Images rgb / out: DEVICE float [B, 3, H, W].  image_ids: HOST int32 [B], the
+ * grid of each image, distinct, in [0, N).
+ *
+ * s3g_bilagrid_slice_forward  <- gsplat lib_bilagrid slice(bil_grids, xy, rgb, grid_idx) at the pixel centres, through
+ *                                BilateralGrid.forward (F.grid_sample, align_corners=True, padding_mode="border")
+ * For pixel (i, j) of image b with colour (r, g, bl): x = (j + 0.5) / W (GX - 1), y = (i + 0.5) / H (GY - 1),
+ * z = (0.299 r + 0.587 g + 0.114 bl) (L - 1), each clamped to [0, size - 1]; A = the trilinear interpolation of grid
+ * image_ids[b] at (x, y, z); out = A[:, :3] (r, g, bl) + A[:, 3].  One launch per 512 images, one thread per pixel; no
+ * intermediate in global memory.  out must not alias rgb.
+ *
+ * s3g_bilagrid_slice_backward  <- the autograd backward of the same formula
+ * With grad_out [B, 3, H, W]: writes grad_rgb [B, 3, H, W] (may be NULL: not computed) and, for every listed image, the
+ * row image_ids[b] of grad_grids [N, 12, L, GY, GX] (stored, not added: the caller zeroes the buffer; other rows are
+ * not touched).  grad_rgb flows through A and through the luminance guide z, whose gradient is 0 where the unclamped
+ * z is <= 0 or >= L - 1 (torch's border rule; so also for L == 1).  Two launches per 512 images: a gather over each
+ * grid cell column's pixel support that writes fixed-order partial sums into the workspace, and their sum in split
+ * order.  No atomics: two calls on the same inputs give bitwise equal results.  workspace:
+ * s3g_bilagrid_slice_backward_workspace_bytes(...) bytes, 16-byte aligned.
+ *
+ * s3g_bilagrid_tv_forward / _backward  <- gsplat total_variation_loss(bil_grids.grids)
+ * loss = (1/N) sum over the axes d in {L, GY, GX} of sum (grids shifted by one along d - grids)^2 / (12 L GY GX (n_d - 1)
+ * / n_d) (an axis of size 1 adds 0).  forward: writes the DEVICE float scalar `loss`; workspace of
+ * s3g_bilagrid_tv_workspace_bytes(...) bytes, 8-byte aligned; two launches, a fixed partition summed in double.
+ * backward: gscale = DEVICE float[1] (the upstream gradient; no host synchronisation), OVERWRITES grad
+ * [N, 12, L, GY, GX] with gscale * d loss / d grids; one launch.
+ *
+ * Every size works (L, GY, GX >= 1; the grid need not fit in shared memory).  S3G_ERR_ARG before any launch: a size
+ * <= 0, a NULL pointer, an id outside [0, N), duplicate ids, N 12 L GY GX or 3 H W above INT_MAX, an unaligned
+ * workspace. */
+int s3g_bilagrid_slice_forward(int N, int L, int GY, int GX, const float* grids, int B, int H, int W,
+                               const int32_t* image_ids, const float* rgb, float* out, void* stream);
+size_t s3g_bilagrid_slice_backward_workspace_bytes(int N, int L, int GY, int GX, int B, int H, int W);
+int s3g_bilagrid_slice_backward(int N, int L, int GY, int GX, const float* grids, int B, int H, int W,
+                                const int32_t* image_ids, const float* rgb, const float* grad_out, float* grad_rgb,
+                                float* grad_grids, void* workspace, void* stream);
+size_t s3g_bilagrid_tv_workspace_bytes(int N, int L, int GY, int GX);
+int s3g_bilagrid_tv_forward(int N, int L, int GY, int GX, const float* grids, float* loss, void* workspace,
+                            void* stream);
+int s3g_bilagrid_tv_backward(int N, int L, int GY, int GX, const float* grids, const float* gscale, float* grad,
+                             void* stream);
+
 /* ---- densify / prune row gather -----------------------------------------------------------
  * s3g_gather_rows  <- _prune_optimizer / cat_tensors_to_optimizer / prune_points / densification_postfix
  *                     scene/gaussian_model.py:411-470 (boolean indexing + torch.cat per tensor)

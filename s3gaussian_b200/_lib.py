@@ -105,6 +105,13 @@ SIGNATURES = {
     "s3g_plane_reg_forward": (_I, [_I, _V, _V, _V, _V]),
     "s3g_plane_reg_backward": (_I, [_I, _V, _V, _V]),
     "s3g_image_loss_backward": (_I, [_I, _I, _I, _I, _V, _V, _V, _V, _F, _V, _V, _V, _V, _V, _V]),
+    # bilateral grids: (N, L, GY, GX, grids, ...); image_ids is a HOST int32 array
+    "s3g_bilagrid_slice_forward": (_I, [_I, _I, _I, _I, _V, _I, _I, _I, _V, _V, _V, _V]),
+    "s3g_bilagrid_slice_backward_workspace_bytes": (_SZ, [_I, _I, _I, _I, _I, _I, _I]),
+    "s3g_bilagrid_slice_backward": (_I, [_I, _I, _I, _I, _V, _I, _I, _I, _V, _V, _V, _V, _V, _V, _V]),
+    "s3g_bilagrid_tv_workspace_bytes": (_SZ, [_I, _I, _I, _I]),
+    "s3g_bilagrid_tv_forward": (_I, [_I, _I, _I, _I, _V, _V, _V, _V]),
+    "s3g_bilagrid_tv_backward": (_I, [_I, _I, _I, _I, _V, _V, _V, _V]),
 }
 
 
