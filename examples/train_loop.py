@@ -3,6 +3,7 @@ train.py (scene_reconstruction, train.py:330-530) with every heavy step running 
 
     python examples/train_loop.py [--points 200000] [--iters 300] [--fine] [--filter-3d] [--densify-until N]
                                  [--absgrad-threshold T | --mcmc-cap N] [--sparse-adam] [--bilateral-grid]
+                                 [--sky]
 
 Synthetic data (there is no dataset reader here): a random cloud initialised through create_from_pcd
 (3-NN scales), targets rendered from a perturbed copy of it.  Needs a CUDA device (sm_90a).
@@ -19,6 +20,15 @@ import torch
 from s3gaussian_b200 import losses, synthetic as syn
 from s3gaussian_b200.gaussian_model import GaussianModel, default_optimization_params
 from s3gaussian_b200.gaussian_renderer import PipelineParams, render
+
+
+def sky_directions(c2w, K, H, W):
+    """Unit world-space ray directions [3, H, W] of the pixel grid (the sky model's step 1), float32 torch."""
+    y, x = torch.meshgrid(torch.arange(H, device=c2w.device, dtype=torch.float32),
+                          torch.arange(W, device=c2w.device, dtype=torch.float32), indexing="ij")
+    cam = torch.stack([(x - K[0, 2] + 0.5) / K[0, 0], (y - K[1, 2] + 0.5) / K[1, 1], torch.ones_like(x)])
+    d = torch.einsum("ij,jhw->ihw", c2w[:3, :3], cam)
+    return d / (d.norm(dim=0, keepdim=True) + 1e-8)
 
 
 def main():
@@ -45,7 +55,13 @@ def main():
                     help="per-camera bilateral-grid colour correction (gsplat --use_bilateral_grid): every camera's "
                          "targets get a fixed exposure difference, and each render is sliced through its camera's "
                          "grid before the loss")
+    ap.add_argument("--sky", action="store_true",
+                    help="sky model (the reference's Background_Model(model_type='mlp')): the targets get an analytic, "
+                         "direction-dependent sky behind the Gaussians; each render (zero background, alpha image) is "
+                         "composited over the model's sky, and alpha is pulled towards 1 - the sky mask")
     a = ap.parse_args()
+    if a.sky and a.bilateral_grid:
+        ap.error("--sky re-renders the targets over its sky, which would drop --bilateral-grid's exposure changes")
     if a.mcmc_cap and a.absgrad_threshold > 0:
         ap.error("--mcmc-cap replaces densify / prune, so --absgrad-threshold has nothing to select")
     if not torch.cuda.is_available():
@@ -83,6 +99,25 @@ def main():
         # gsplat's schedule (its LinearLR and ExponentialLR chained, so their factors multiply): lr 2e-3, a linear
         # warm-up from 0.01x over the first 1000 iterations and an exponential decay to 0.01x at the last iteration
         bil_opt = FusedAdam([{"params": [bil_grids.grids], "lr": 2e-3, "name": "bilagrid"}], lr=2e-3, eps=1e-15)
+    sky_model = sky_opt = None
+    if a.sky:
+        from s3gaussian_b200.optim import FusedAdam
+        from s3gaussian_b200.sky import Background_Model, sky_camera
+        # the ground truth's sky: a smooth colour of the world-space ray direction, behind the truth cloud; the sky
+        # mask is where the truth's alpha is below 0.5
+        opa_pipe = PipelineParams()
+        opa_pipe.render_opacity = True
+        with torch.no_grad():
+            for k, c in enumerate(cams):
+                out = render(c, gt, opa_pipe, bg, stage="coarse")
+                v = sky_directions(*sky_camera(c), a.height, a.width)
+                sky = torch.stack([0.45 + 0.35 * v[2], 0.6 + 0.25 * v[2] - 0.1 * v[0], 0.85 - 0.1 * v[1]]).clamp(0, 1)
+                alpha = out["alpha"]
+                targets[k] = (out["render"] + (1.0 - alpha) * sky, targets[k][1], (alpha < 0.5).float())
+        train_pipe.render_opacity = True
+        sky_model = Background_Model(img_width=a.width, img_height=a.height, model_cfg={"mlp_width": 64}).to(dev)
+        # not tuned on real data: the learning rate and the mask-loss weight below only have to work on this scene
+        sky_opt = FusedAdam([{"params": list(sky_model.parameters()), "lr": 1e-3, "name": "sky"}], lr=1e-3, eps=1e-15)
     colours = (truth.features_dc[:, 0] * 0.28209479177387814 + 0.5).clamp(0, 1)
     pcd = SimpleNamespace(points=truth.xyz.numpy(), colors=colours.numpy())
 
@@ -112,10 +147,16 @@ def main():
         image, depth = out["render"], out["depth"]
         if bil_grids is not None:
             image = bil_grids.slice(image, k)
+        if sky_model is not None:     # bg is zero: image + (1 - alpha) sky is the render over a per-pixel sky
+            alpha = out["alpha"]
+            image = image + (1.0 - alpha) * sky_model(*sky_camera(cams[k]))
         l1, ssim_value, depth_l2 = losses.image_loss_terms(image, targets[k][0], depth, targets[k][1])
         loss = l1 + 0.5 * depth_l2 + 0.2 * (1.0 - ssim_value)                    # train.py:395-419
         if bil_grids is not None:
             loss = loss + 10.0 * bil_grids.tv_loss()
+        if sky_model is not None:     # binary cross-entropy of alpha against 1 - sky mask
+            loss = loss + 0.05 * torch.nn.functional.binary_cross_entropy(alpha.clamp(1e-6, 1 - 1e-6),
+                                                                          1.0 - targets[k][2])
         if a.fine:
             loss = loss + 0.001 * out["dx"].abs().mean() + 0.001 * out["dshs"].abs().mean() + \
                 gaussians.compute_regulation(0.01, 0.0001, 0.0001)
@@ -152,6 +193,9 @@ def main():
             bil_opt.param_groups[0]["lr"] = 2e-3 * warm * decay
             bil_opt.step()
             bil_opt.zero_grad(set_to_none=True)
+        if sky_opt is not None:
+            sky_opt.step()
+            sky_opt.zero_grad(set_to_none=True)
         if a.mcmc_cap:
             gaussians.inject_noise(xyz_lr)
         if it % 50 == 0:

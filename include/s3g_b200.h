@@ -782,6 +782,47 @@ int s3g_bilagrid_tv_forward(int N, int L, int GY, int GX, const float* grids, fl
 int s3g_bilagrid_tv_backward(int N, int L, int GY, int GX, const float* grids, const float* gscale, float* grad,
                              void* stream);
 
+/* ---- sky model (EmerNeRF's sky head; scene/background_model.py SkyModel, Background_Model(model_type="mlp")) --------
+ * A direction MLP behind the Gaussians.  For pixel (x, y) of an H x W image, R = c2w[:3, :3]:
+ *   d = R ((x - cx + 0.5) / fx, (y - cy + 0.5) / fy, 1),  v = d / (|d| + 1e-8)
+ *   enc = [v, sin(xb), sin(xb + pi/2)], xb = (v, 2v, 4v, 8v, 16v) scale-major          (33 features)
+ *   h1 = relu(W0 enc + b0), h2 = relu(W1 [h1, enc] + b1), sky = sigmoid(W2 h2 + b2)
+ * Weights in PyTorch's fp32 layout: W0 [width, 33], W1 [width, width + 33], W2 [3, width]; width = 64, 128, 192 or
+ * 256.  c2w: DEVICE float [4, 4] row-major, intrinsic: DEVICE float [3, 3] ((fx, 0, cx), (0, fy, cy), (0, 0, 1)); no
+ * host synchronisation.  The parameters are read on every call (no prepared copy outlives a call).
+ *
+ * s3g_sky_forward   writes out_sky [3, H, W].  The wide layers run as 3xTF32 mma.sync; nothing per pixel but the output
+ *                   is written to global memory.
+ * s3g_sky_backward  with dL_dsky [3, H, W], writes (stores; the caller does not zero them) every weight and bias
+ *                   gradient.  No gradient for the camera.  Recomputes the forward in chunks of 65536 pixels inside the
+ *                   workspace; the weight gradients are fixed-order sums of per-CTA partials, so two calls give bitwise
+ *                   equal results.
+ * workspace: s3g_sky_workspace_bytes(width, H, W) bytes (0 for invalid sizes), 16-byte aligned; one buffer serves both
+ * calls.  S3G_ERR_ARG before any launch: a width that is not a multiple of 64 in [64, 256], H < 1 or W < 1, 3 H W above
+ * INT_MAX, a NULL pointer, a NULL or unaligned workspace. */
+typedef struct s3g_sky_net {
+    int width;
+    const float* w0;   /* [width, 33] */
+    const float* b0;   /* [width] */
+    const float* w1;   /* [width, width + 33] */
+    const float* b1;   /* [width] */
+    const float* w2;   /* [3, width] */
+    const float* b2;   /* [3] */
+} s3g_sky_net;
+typedef struct s3g_sky_net_grads {
+    float* w0;
+    float* b0;
+    float* w1;
+    float* b1;
+    float* w2;
+    float* b2;
+} s3g_sky_net_grads;
+size_t s3g_sky_workspace_bytes(int width, int H, int W);
+int s3g_sky_forward(const s3g_sky_net* net, int H, int W, const float* c2w, const float* intrinsic, float* out_sky,
+                    void* workspace, void* stream);
+int s3g_sky_backward(const s3g_sky_net* net, int H, int W, const float* c2w, const float* intrinsic,
+                     const float* dL_dsky, const s3g_sky_net_grads* grads, void* workspace, void* stream);
+
 /* ---- densify / prune row gather -----------------------------------------------------------
  * s3g_gather_rows  <- _prune_optimizer / cat_tensors_to_optimizer / prune_points / densification_postfix
  *                     scene/gaussian_model.py:411-470 (boolean indexing + torch.cat per tensor)

@@ -112,7 +112,23 @@ SIGNATURES = {
     "s3g_bilagrid_tv_workspace_bytes": (_SZ, [_I, _I, _I, _I]),
     "s3g_bilagrid_tv_forward": (_I, [_I, _I, _I, _I, _V, _V, _V, _V]),
     "s3g_bilagrid_tv_backward": (_I, [_I, _I, _I, _I, _V, _V, _V, _V]),
+    # sky model: the net and its gradients are a SkyNet / SkyNetGrads (below) with ctypes.byref()
+    "s3g_sky_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "s3g_sky_forward": (_I, [_V, _I, _I, _V, _V, _V, _V, _V]),
+    "s3g_sky_backward": (_I, [_V, _I, _I, _V, _V, _V, _V, _V, _V]),
 }
+
+
+class SkyNet(C.Structure):
+    """s3g_sky_net (include/s3g_b200.h)."""
+    _fields_ = [("width", C.c_int), ("w0", C.c_void_p), ("b0", C.c_void_p), ("w1", C.c_void_p), ("b1", C.c_void_p),
+                ("w2", C.c_void_p), ("b2", C.c_void_p)]
+
+
+class SkyNetGrads(C.Structure):
+    """s3g_sky_net_grads (include/s3g_b200.h)."""
+    _fields_ = [("w0", C.c_void_p), ("b0", C.c_void_p), ("w1", C.c_void_p), ("b1", C.c_void_p), ("w2", C.c_void_p),
+                ("b2", C.c_void_p)]
 
 
 class AdamTensor(C.Structure):

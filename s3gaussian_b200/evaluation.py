@@ -142,7 +142,8 @@ def flow_colors(dx_to: torch.Tensor, dx_from: torch.Tensor, normalize: bool = Fa
 
 
 def render_pixels(viewpoint_stack, gaussians, bg, pipe, compute_metrics: bool = True,
-                  return_decomposition: bool = True, debug: bool = False, lpips_fn=None, with_opacity: bool = False):
+                  return_decomposition: bool = True, debug: bool = False, lpips_fn=None, with_opacity: bool = False,
+                  sky_model=None):
     """Drop-in for utils/video_utils.py:render_pixels: renders every camera of `viewpoint_stack` (the fine stage,
     under no_grad) and returns the reference's result dict:
 
@@ -165,6 +166,11 @@ def render_pixels(viewpoint_stack, gaussians, bg, pipe, compute_metrics: bool = 
     min-max normalises the flow colours, as the reference's.  lpips is -1 unless `lpips_fn(rgb, gt)` (-> tensor) is
     given; s3gaussian_b200.lpips.LPIPS() computes the reference's LPIPS on the device.  Not covered: save_seperate_pcd (render_func
     :243-249), which render_pixels never enables.
+
+    sky_model (a s3gaussian_b200.sky.Background_Model at the views' image size): each view's rgbs image, and the
+    PSNR / SSIM / LPIPS computed on it, is the render over a zero background plus (1 - alpha) times the view's sky
+    (sky.sky_camera gives its c2w / intrinsic); the alpha image comes from the same walk.  The static / dynamic
+    images are unchanged.
     """
     from .gaussian_renderer import dynamic_mask_of, fine_front, pipe_rasterizer_kwargs, raster_settings_for
     from .diff_gaussian_rasterization import GaussianRasterizer
@@ -207,8 +213,14 @@ def render_pixels(viewpoint_stack, gaussians, bg, pipe, compute_metrics: bool = 
             out = GaussianRasterizer(raster_settings=rs, **pipe_rasterizer_kwargs(pipe)).forward_eval(
                 means3D=means3D, means2D=torch.zeros_like(means3D), opacities=opacity, group=group,
                 flow_colors=[colours[a] for a in need], shs=shs, colors_precomp=colors_precomp, scales=scales,
-                rotations=rotations, **({"with_opacity": True} if with_opacity else {}))
+                rotations=rotations, **({"with_opacity": True} if with_opacity or sky_model is not None else {}))
             rgb, _, depth_t, decomposition, flows = out[:5]
+            if sky_model is not None:
+                # rgb = render_bg0 + (1 - alpha) bg (the forward-opacity contract), so the sky composite swaps bg out
+                from .sky import sky_camera
+                alpha = out[5][0]
+                sky = sky_model(*sky_camera(cam))
+                rgb = rgb + (1.0 - alpha) * (sky - rs.bg.reshape(-1, 1, 1))
             if with_opacity:
                 alpha, median, alpha_d, alpha_s = out[5]
                 opacities.append(alpha[0].cpu().numpy())
