@@ -31,6 +31,16 @@ def sky_directions(c2w, K, H, W):
     return d / (d.norm(dim=0, keepdim=True) + 1e-8)
 
 
+def lens_camera(cam):
+    """cam with a principal point 3 % of the width right and 2 % of the height up of the centre, and mild barrel
+    distortion with tangential terms (the K convention of render(pipe.lens): pixel centres at j + 0.5)."""
+    W, H = cam.image_width, cam.image_height
+    fx, fy = W / (2 * cam.tanfovx), H / (2 * cam.tanfovy)
+    K = torch.tensor([[fx, 0.0, 0.53 * W], [0.0, fy, 0.48 * H], [0.0, 0.0, 1.0]])
+    return syn.SyntheticCamera(W, H, cam.FoVx, cam.FoVy, cam.world_view_transform, cam.full_proj_transform,
+                               cam.camera_center, cam.time, K, torch.tensor([-0.1, 0.02, 5e-4, -3e-4, 0.0]))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--points", type=int, default=200_000)
@@ -59,6 +69,10 @@ def main():
                     help="sky model (the reference's Background_Model(model_type='mlp')): the targets get an analytic, "
                          "direction-dependent sky behind the Gaussians; each render (zero background, alpha image) is "
                          "composited over the model's sky, and alpha is pulled towards 1 - the sky mask")
+    ap.add_argument("--lens", action="store_true",
+                    help="camera intrinsics and distortion: every camera gets an off-centre principal point and OpenCV "
+                         "radial-tangential coefficients; the targets and the training renders go through them "
+                         "(pipe.lens)")
     a = ap.parse_args()
     if a.sky and a.bilateral_grid:
         ap.error("--sky re-renders the targets over its sky, which would drop --bilateral-grid's exposure changes")
@@ -74,6 +88,9 @@ def main():
     train_pipe = PipelineParams()
     train_pipe.filter_3d = a.filter_3d
     train_pipe.absgrad = a.absgrad_threshold > 0
+    if a.lens:
+        cams = [lens_camera(c) for c in cams]
+        pipe.lens = train_pipe.lens = True
 
     # ---- scene: "ground truth" cloud -> target images; training starts from a point cloud of it -------
     truth = syn.make_cloud(a.points, seed=0)

@@ -318,6 +318,48 @@ int s3g_rasterize_backward_absgrad(const s3g_raster_scene* scene, const s3g_rast
                                    void* workspace /* deterministic: as s3g_rasterize_backward_deterministic */,
                                    void* stream);
 
+/* ---- camera intrinsics and lens distortion (OpenCV radial-tangential) ---------------------------------------------
+ * Not in the reference, which projects through the symmetric pinhole of tan_fovx / tan_fovy (principal point at the
+ * image centre, no distortion); gsplat and upstream 3DGS forks take K and OpenCV distortion.  Street-scene cameras
+ * (Waymo) have an off-centre principal point and five distortion coefficients.
+ * The lens, in pixels of the render size: fx, fy, cx, cy, k1, k2, p1, p2, k3.  K convention: pixel j's centre is at
+ * j + 0.5, so a centred camera has cx = width / 2 (the sky model's convention); an OpenCV K, whose pixel centres are
+ * at j, needs cx + 0.5 and cy + 0.5.  For a Gaussian with camera-space mean t = view . p:
+ *   1. near cull as before: t.z <= 0.2 is invisible;
+ *   2. x = t.x / t.z, y = t.y / t.z, s = x^2 + y^2, rho = 1 + k1 s + k2 s^2 + k3 s^3,
+ *      xd = x rho + 2 p1 x y + p2 (s + 2 x^2),  yd = y rho + p1 (s + 2 y^2) + 2 p2 x y;
+ *   3. lens cull: s* is the smallest positive root of 1 + 3 k1 s + 5 k2 s^2 + 7 k3 s^3, the radius where the radial
+ *      map r rho(r^2) stops increasing; where it exists, s > s* is culled (radius 0), since beyond it the polynomial
+ *      folds points from outside the frustum back into the image.  The tangential terms do not enter the bound.
+ *      s3g_lens_max_radius2 returns s* (computed in double, as the forward does once per call), or +inf;
+ *   4. mean2D = (fx xd + cx - 0.5, fy yd + cy - 0.5) in the rasterizer's pixel coordinates; dL_dmean2D keeps its
+ *      units, the gradient with respect to (2 u + 1) / width - 1 (and likewise v);
+ *   5. the 2-D covariance is (F D J_n) W Sigma W^T (F D J_n)^T, then the 0.3 px^2 dilation and, antialiased, the
+ *      filter as above.  F = diag(fx, fy); J_n = [[1/z, 0, -x_c/z], [0, 1/z, -y_c/z]] with x_c, y_c = x, y clamped
+ *      to [-1.3 cx/fx, 1.3 (width - cx)/fx] and [-1.3 cy/fy, 1.3 (height - cy)/fy] (the plain 1.3 tanfov when
+ *      cx = width / 2); D = d(xd, yd)/d(x, y) at the unclamped (x, y).  With zero coefficients D = I and, with
+ *      fx = width / (2 tan_fovx), cx = width / 2 (likewise y), this is the plain forward's projection;
+ *   6. depth, SH colour, radii, tile rectangles and the composite follow as in the plain forward.
+ * viewmatrix still places the camera; projmatrix and tan_fovx / tan_fovy are not used by the projection.
+ * s3g_rasterize_forward_lens is s3g_rasterize_forward_opacity (`opa` may be NULL: s3g_rasterize_forward) or, with
+ * antialiased != 0, s3g_rasterize_forward_antialiased, through the lens: the same scene, arguments, contract and
+ * extras (aux pair, decomposition, flow sets, opacity images).  The library remembers per geometry buffer the lens of
+ * its last forward (every forward updates that record), and s3g_rasterize_backward, its deterministic, *_opacity and
+ * absgrad forms then apply the chain rule of that projection: the mean's path through D^T F, the covariance's through
+ * F D J_n with D's own dependence on the mean.  The lens gets no gradient.
+ * S3G_ERR_ARG before any launch: every case of the call it extends; a NULL lens; fx or fy not finite and positive; cx,
+ * cy or a coefficient not finite; after a lens forward, s3g_rasterize_camera_backward (camera gradients through the
+ * lens are not implemented) and a backward with a peer sink (the fused gradient exchange does not take its
+ * gradients). */
+typedef struct s3g_raster_lens {
+    float fx, fy, cx, cy;
+    float k1, k2, p1, p2, k3;
+} s3g_raster_lens;
+int64_t s3g_rasterize_forward_lens(const s3g_raster_scene* scene, const s3g_raster_forward_args* fwd,
+                                   const s3g_raster_opacity_args* opa /* may be NULL */, int antialiased,
+                                   const s3g_raster_lens* lens, void* stream);
+double s3g_lens_max_radius2(const s3g_raster_lens* lens);
+
 /* ---- 3-D smoothing filter (Mip-Splatting's compute_3D_filter, get_scaling / get_opacity_with_3D_filter) ----------
  * Not in the reference.  Extends the model side of render(): optimisation lets a Gaussian shrink far below the finest
  * sampling interval any training camera had at its position, and a view closer than every training camera (a lane

@@ -39,6 +39,9 @@ SIGNATURES = {
     # the backward with the absolute screen-space gradients: RasterOpacityArgs or NULL, dL_dmean2D_abs, deterministic,
     # workspace
     "s3g_rasterize_backward_absgrad": (_I, [_V, _V, _V, _V, _I, _V, _V]),
+    # the forward through a camera's intrinsics and lens distortion: RasterOpacityArgs or NULL, antialiased, RasterLens
+    "s3g_rasterize_forward_lens": (_I64, [_V, _V, _V, _I, _V, _V]),
+    "s3g_lens_max_radius2": (_D, [_V]),
     "s3g_filter3d_compute_workspace_bytes": (_SZ, [_I]),
     "s3g_filter3d_compute": (_I, [_I, _V, _I, _V, _V, _V, _V, _V]),
     "s3g_filter3d_apply_forward": (_I, [_I, _V, _V, _V, _V, _V, _V]),
@@ -230,6 +233,11 @@ class RasterOpacityArgs(C.Structure):
     """s3g_raster_opacity_args (include/s3g_b200.h)."""
     _fields_ = [("out_alpha", C.c_void_p), ("out_median_depth", C.c_void_p), ("out_alpha_d", C.c_void_p),
                 ("out_alpha_s", C.c_void_p), ("dL_dpix_alpha", C.c_void_p), ("dL_dpix_median", C.c_void_p)]
+
+
+class RasterLens(C.Structure):
+    """s3g_raster_lens (include/s3g_b200.h)."""
+    _fields_ = [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "k1", "k2", "p1", "p2", "k3")]
 
 
 class RasterCameraGrads(C.Structure):

@@ -12,6 +12,7 @@
 #include <cstring>
 #include <mutex>
 #include <string>
+#include <unordered_map>
 #include <unordered_set>
 #include <vector>
 
@@ -312,6 +313,95 @@ bool has_aa_state(const char* geom) {
     return g_aa_states.count(geom) != 0;
 }
 
+// Geometry buffers whose last forward went through a lens (s3g_rasterize_forward_lens), with that lens: the backward
+// applies its chain rule, chosen on the host before any launch.  Every forward on a buffer updates its entry; no cap,
+// for the reason of the antialiasing record.
+std::mutex g_lens_mu;
+std::unordered_map<const char*, LensParams> g_lens_states;
+
+void note_lens_state(const char* geom, const LensParams* lens) {
+    std::lock_guard<std::mutex> lock(g_lens_mu);
+    if (lens) g_lens_states[geom] = *lens;
+    else g_lens_states.erase(geom);
+}
+bool lens_state(const char* geom, LensParams* out) {
+    if (!geom) return false;
+    std::lock_guard<std::mutex> lock(g_lens_mu);
+    auto it = g_lens_states.find(geom);
+    if (it == g_lens_states.end()) return false;
+    if (out) *out = it->second;
+    return true;
+}
+
+// s*: the smallest positive root of 1 + 3 k1 s + 5 k2 s^2 + 7 k3 s^3 = d(r rho(r^2))/dr, in double, or +inf.  The
+// polynomial is monotone between its critical points; the first interval whose end is not positive holds the root,
+// found by bisection.
+double lens_max_radius2(double k1, double k2, double k3) {
+    const double c[4] = {1.0, 3.0 * k1, 5.0 * k2, 7.0 * k3};
+    auto p = [&](double s) { return c[0] + s * (c[1] + s * (c[2] + s * c[3])); };
+    int deg = 3;
+    while (deg > 0 && c[deg] == 0.0) --deg;
+    if (deg == 0) return INFINITY;
+    double bound = 0.0;   // Cauchy: every root has |s| < 1 + max |c_i / c_deg|
+    for (int i = 0; i < deg; ++i) bound = std::max(bound, std::fabs(c[i] / c[deg]));
+    bound += 1.0;
+    // positive roots of p' = c1 + 2 c2 s + 3 c3 s^2, ascending
+    std::vector<double> ends;
+    const double qa = 3.0 * c[3], qb = 2.0 * c[2], qc = c[1];
+    if (qa != 0.0) {
+        const double disc = qb * qb - 4.0 * qa * qc;
+        if (disc >= 0.0) {
+            const double r = std::sqrt(disc);
+            const double q = -0.5 * (qb + (qb >= 0.0 ? r : -r));
+            if (q != 0.0) {
+                ends.push_back(q / qa);
+                ends.push_back(qc / q);
+            } else {
+                ends.push_back(0.0);
+            }
+        }
+    } else if (qb != 0.0) {
+        ends.push_back(-qc / qb);
+    }
+    std::sort(ends.begin(), ends.end());
+    std::vector<double> pts = {0.0};
+    for (double e : ends)
+        if (e > 0.0 && e < bound) pts.push_back(e);
+    pts.push_back(bound);
+    for (size_t i = 0; i + 1 < pts.size(); ++i) {
+        double lo = pts[i], hi = pts[i + 1];
+        if (p(hi) > 0.0) continue;   // p(lo) > 0 here: no root yet
+        for (int it = 0; it < 400 && lo < hi; ++it) {
+            const double mid = 0.5 * (lo + hi);
+            if (mid <= lo || mid >= hi) break;
+            if (p(mid) > 0.0) lo = mid;
+            else hi = mid;
+        }
+        return hi;
+    }
+    return INFINITY;
+}
+
+// The kernels' LensParams of a lens and an image size; S3G_ERR_ARG for a lens s3g_rasterize_forward_lens rejects.
+int lens_params(const s3g_raster_lens* l, int width, int height, LensParams* out) {
+    if (!l) return fail(S3G_ERR_ARG, "forward_lens: null lens");
+    if (!(std::isfinite(l->fx) && l->fx > 0.f && std::isfinite(l->fy) && l->fy > 0.f))
+        return fail(S3G_ERR_ARG, "forward_lens: fx and fy must be finite and positive");
+    for (float v : {l->cx, l->cy, l->k1, l->k2, l->p1, l->p2, l->k3})
+        if (!std::isfinite(v)) return fail(S3G_ERR_ARG, "forward_lens: cx, cy and the distortion coefficients must be finite");
+    LensParams& L = *out;
+    L.fx = l->fx; L.fy = l->fy; L.cx = l->cx; L.cy = l->cy;
+    L.k1 = l->k1; L.k2 = l->k2; L.p1 = l->p1; L.p2 = l->p2; L.k3 = l->k3;
+    L.max_r2 = (float)lens_max_radius2(l->k1, l->k2, l->k3);
+    L.xlo = (float)(-1.3 * (double)l->cx / l->fx);
+    L.xhi = (float)(1.3 * ((double)width - l->cx) / l->fx);
+    L.ylo = (float)(-1.3 * (double)l->cy / l->fy);
+    L.yhi = (float)(1.3 * ((double)height - l->cy) / l->fy);
+    L.ndc_x = 2.f / (float)width;
+    L.ndc_y = 2.f / (float)height;
+    return S3G_OK;
+}
+
 // one forward composite walk; the plain walks take the RenderFwdArgs part of ra, and an opacity walk is launched when
 // opa is given
 template <int NA, bool SPLIT>
@@ -322,8 +412,9 @@ void launch_render_forward(const RenderSplitArgs& ra, const AuxSet& a1, const Op
 }
 
 // o: the opacity outputs (s3g_rasterize_forward_opacity), or NULL for the plain forward.  aa: antialiased
+// lens: the lens forward's parameters (s3g_rasterize_forward_lens), or NULL
 int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f, const s3g_raster_opacity_args* o,
-                     bool aa, cudaStream_t stream) {
+                     bool aa, cudaStream_t stream, const LensParams* lens = nullptr) {
     const int P = s.P, width = s.width, height = s.height, debug = s.debug;
     if (P < 0 || width <= 0 || height <= 0) return fail(S3G_ERR_ARG, "forward: bad sizes");
     if (!f.geom_alloc || !f.binning_alloc || !f.image_alloc) return fail(S3G_ERR_ARG, "forward: null allocator");
@@ -399,6 +490,7 @@ int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f
     if (!gptr) return fail(S3G_ERR_ALLOC, "forward: geometry allocator returned NULL");
     GeomState geom = GeomState::carve(gptr, P);
     note_aa_state(gptr, aa);
+    note_lens_state(gptr, lens);
     char* iptr = f.image_alloc(f.image_user, s3g_image_bytes(width, height));
     if (!iptr) return fail(S3G_ERR_ALLOC, "forward: image allocator returned NULL");
     ImageState img = ImageState::carve(iptr, width, height);
@@ -432,10 +524,22 @@ int64_t forward_impl(const s3g_raster_scene& s, const s3g_raster_forward_args& f
     {
         const int grid = (P + PRE_THREADS - 1) / PRE_THREADS;
         const bool use_sh = s.colors_precomp == nullptr;
-        const int rc = aa ? launch_sh_rows(preprocess_forward_kernel<16, true>, preprocess_forward_kernel<0, true>, pa,
-                                           grid, PRE_THREADS, s.M, use_sh, "forward", stream)
-                          : launch_sh_rows(preprocess_forward_kernel<16>, preprocess_forward_kernel<0>, pa, grid,
-                                           PRE_THREADS, s.M, use_sh, "forward", stream);
+        int rc;
+        if (lens) {
+            PreFwdLensArgs pl;
+            static_cast<PreFwdArgs&>(pl) = pa;
+            pl.lens = *lens;
+            rc = aa ? launch_sh_rows(preprocess_forward_lens_kernel<16, true>, preprocess_forward_lens_kernel<0, true>,
+                                     pl, grid, PRE_THREADS, s.M, use_sh, "forward", stream)
+                    : launch_sh_rows(preprocess_forward_lens_kernel<16, false>,
+                                     preprocess_forward_lens_kernel<0, false>, pl, grid, PRE_THREADS, s.M, use_sh,
+                                     "forward", stream);
+        } else {
+            rc = aa ? launch_sh_rows(preprocess_forward_kernel<16, true>, preprocess_forward_kernel<0, true>, pa,
+                                     grid, PRE_THREADS, s.M, use_sh, "forward", stream)
+                    : launch_sh_rows(preprocess_forward_kernel<16>, preprocess_forward_kernel<0>, pa, grid,
+                                     PRE_THREADS, s.M, use_sh, "forward", stream);
+        }
         if (rc != S3G_OK) return rc;
     }
     S3G_STAGE("preprocess_forward");
@@ -643,6 +747,10 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
     if (sink && aa)
         return fail(S3G_ERR_ARG, "backward_dp: the fused gradient exchange does not take an antialiased forward's "
                                  "gradients");
+    LensParams lens;
+    const bool use_lens = lens_state(b.geom_buffer, &lens);
+    if (sink && use_lens)
+        return fail(S3G_ERR_ARG, "backward_dp: the fused gradient exchange does not take a lens forward's gradients");
     if ((b.dL_dpix_aux != nullptr) != (b.dL_dcolor_aux != nullptr))
         return fail(S3G_ERR_ARG, "backward: dL_dpix_aux and dL_dcolor_aux go together");
     const bool use_aux = b.dL_dpix_aux != nullptr;
@@ -737,7 +845,18 @@ int backward_impl(const s3g_raster_scene& s, const s3g_raster_backward_args& b, 
     }
     {
         const int grid = (P + PRE_THREADS - 1) / PRE_THREADS;
-        const int rc = sink ? launch_sh_rows(preprocess_backward_kernel<16, true>, preprocess_backward_kernel<0, true>,
+        PreBwdLensArgs pbl;
+        if (use_lens) {
+            static_cast<PreBwdArgs&>(pbl) = pb;
+            pbl.lens = lens;
+        }
+        const int rc = use_lens ? (aa ? launch_sh_rows(preprocess_backward_lens_kernel<16, true>,
+                                                       preprocess_backward_lens_kernel<0, true>, pbl, grid,
+                                                       PRE_THREADS, s.M, use_sh, "backward", stream)
+                                      : launch_sh_rows(preprocess_backward_lens_kernel<16, false>,
+                                                       preprocess_backward_lens_kernel<0, false>, pbl, grid,
+                                                       PRE_THREADS, s.M, use_sh, "backward", stream))
+                       : sink ? launch_sh_rows(preprocess_backward_kernel<16, true>, preprocess_backward_kernel<0, true>,
                                              pb, grid, PRE_THREADS, s.M, use_sh, "backward", stream)
                        : aa ? launch_sh_rows(preprocess_backward_kernel<16, false, true>,
                                              preprocess_backward_kernel<0, false, true>, pb, grid, PRE_THREADS, s.M,
@@ -775,6 +894,21 @@ int64_t s3g_rasterize_forward_antialiased(const s3g_raster_scene* scene, const s
                                           const s3g_raster_opacity_args* opa, void* stream) {
     if (!scene || !fwd) return fail(S3G_ERR_ARG, "forward_antialiased: null scene / forward arguments");
     return forward_impl(*scene, *fwd, opa, true, static_cast<cudaStream_t>(stream));
+}
+
+int64_t s3g_rasterize_forward_lens(const s3g_raster_scene* scene, const s3g_raster_forward_args* fwd,
+                                   const s3g_raster_opacity_args* opa, int antialiased, const s3g_raster_lens* lens,
+                                   void* stream) {
+    if (!scene || !fwd) return fail(S3G_ERR_ARG, "forward_lens: null scene / forward arguments");
+    LensParams L;
+    const int rc = lens_params(lens, scene->width, scene->height, &L);
+    if (rc != S3G_OK) return rc;
+    return forward_impl(*scene, *fwd, opa, antialiased != 0, static_cast<cudaStream_t>(stream), &L);
+}
+
+double s3g_lens_max_radius2(const s3g_raster_lens* lens) {
+    if (!lens) return NAN;
+    return lens_max_radius2(lens->k1, lens->k2, lens->k3);
 }
 
 int s3g_rasterize_backward(const s3g_raster_scene* scene, const s3g_raster_backward_args* bwd, void* stream) {
@@ -829,6 +963,8 @@ int s3g_rasterize_camera_backward(const s3g_raster_scene* scene, const s3g_raste
         return fail(S3G_ERR_ARG, "camera_backward: the backward must have exported dL_dconic and dL_ddepth");
     if (!out->dL_dviewmatrix && !out->dL_dprojmatrix && !out->dL_dcampos)
         return fail(S3G_ERR_ARG, "camera_backward: no output asked for");
+    if (lens_state(b.geom_buffer, nullptr))
+        return fail(S3G_ERR_ARG, "camera_backward: camera gradients after a lens forward are not implemented");
     if (P < 0 || s.width <= 0 || s.height <= 0) return fail(S3G_ERR_ARG, "camera_backward: bad sizes");
     if (P > 0 && (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 15)))
         return fail(S3G_ERR_ARG, "camera_backward: workspace must be non-NULL and 16-byte aligned");

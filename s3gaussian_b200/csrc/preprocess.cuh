@@ -201,6 +201,111 @@ constexpr float AA_RHO_MIN = 2.5e-5f;
 __device__ __forceinline__ float aa_rho(float a, float b, float c, float det1) { return (a * c - b * b) / det1; }
 __device__ __forceinline__ float aa_scale(float rho) { return sqrtf(fmaxf(rho, AA_RHO_MIN)); }
 
+// The camera's own intrinsics and OpenCV radial-tangential distortion (s3g_rasterize_forward_lens).  For the
+// camera-space mean t: x = t.x / t.z, y = t.y / t.z, s = x^2 + y^2, rho = 1 + k1 s + k2 s^2 + k3 s^3,
+// xd = x rho + 2 p1 x y + p2 (s + 2 x^2), yd = y rho + p1 (s + 2 y^2) + 2 p2 x y and the pixel is
+// (fx xd + cx - 0.5, fy yd + cy - 0.5).  The 2-D covariance takes J = F D J_n: F = diag(fx, fy), D = d(xd, yd)/d(x, y)
+// at the unclamped (x, y), J_n the pinhole Jacobian of (x, y) at the mean clamped to [xlo, xhi] x [ylo, yhi].  The host
+// fills the derived fields (lens_params in api.cu).
+struct LensParams {
+    float fx, fy, cx, cy, k1, k2, p1, p2, k3;
+    float max_r2;                // s*: culled where s > s* (+inf: the radial map never folds back)
+    float xlo, xhi, ylo, yhi;    // the 1.3-frustum clamp of x and y in J_n
+    float ndc_x, ndc_y;          // 2 / W, 2 / H: d(ndc) / d(pixel), the units of dL_dmean2D
+};
+
+// (x, y) and everything the distortion, its Jacobian D = [[D00, D01], [D01, D11]] and D's derivatives need
+struct LensPoint {
+    float x, y, s, rho, drho, ddrho;
+    float xd, yd;
+    float D00, D01, D11;
+};
+__device__ __forceinline__ LensPoint lens_point(const LensParams& L, float x, float y) {
+    LensPoint p;
+    p.x = x;
+    p.y = y;
+    const float s = x * x + y * y;
+    p.s = s;
+    p.rho = 1.f + s * (L.k1 + s * (L.k2 + s * L.k3));
+    p.drho = L.k1 + s * (2.f * L.k2 + 3.f * L.k3 * s);    // d rho / ds
+    p.ddrho = 2.f * L.k2 + 6.f * L.k3 * s;                 // d^2 rho / ds^2
+    p.xd = x * p.rho + 2.f * L.p1 * x * y + L.p2 * (s + 2.f * x * x);
+    p.yd = y * p.rho + L.p1 * (s + 2.f * y * y) + 2.f * L.p2 * x * y;
+    p.D00 = p.rho + 2.f * x * x * p.drho + 2.f * L.p1 * y + 6.f * L.p2 * x;
+    p.D01 = 2.f * x * y * p.drho + 2.f * L.p1 * x + 2.f * L.p2 * y;
+    p.D11 = p.rho + 2.f * y * y * p.drho + 6.f * L.p1 * y + 2.f * L.p2 * x;
+    return p;
+}
+
+// ewa_jacobian's lens form: e.t is the camera-space mean with x, y clamped to the lens's limits, e.J = F D J_n (rows as
+// ewa_jacobian's), e.T = W J; p holds the unclamped point.
+struct LensJacobian {
+    EwaJacobian e;
+    LensPoint p;
+};
+__device__ __forceinline__ LensJacobian lens_jacobian(const LensParams& L, const float3& t_view, const float* view) {
+    LensJacobian lj;
+    const float x = t_view.x / t_view.z;
+    const float y = t_view.y / t_view.z;
+    lj.p = lens_point(L, x, y);
+    EwaJacobian& e = lj.e;
+    float3 t = t_view;
+    t.x = min(L.xhi, max(L.xlo, x)) * t.z;
+    t.y = min(L.yhi, max(L.ylo, y)) * t.z;
+    e.t = t;
+    e.x_grad_mul = x < L.xlo || x > L.xhi ? 0.f : 1.f;
+    e.y_grad_mul = y < L.ylo || y > L.yhi ? 0.f : 1.f;
+    const float iz = 1.f / t.z;
+    const float n02 = -t.x * iz * iz, n12 = -t.y * iz * iz;   // J_n = [[1/z, 0, n02], [0, 1/z, n12]]
+    const float a00 = L.fx * lj.p.D00, a01 = L.fx * lj.p.D01, a10 = L.fy * lj.p.D01, a11 = L.fy * lj.p.D11;
+    e.J = m3(a00 * iz, a01 * iz, a00 * n02 + a01 * n12, a10 * iz, a11 * iz, a10 * n02 + a11 * n12, 0.f, 0.f, 0.f);
+    e.W = m3(view[0], view[4], view[8], view[1], view[5], view[9], view[2], view[6], view[10]);
+    e.T = m3_mul(e.W, e.J);
+    return lj;
+}
+
+// the EWA 2-D covariance {a, b, c} of T = W J
+__device__ __forceinline__ float3 cov2d_of_T(const M3& T, const float* cov3D) {
+    const M3 cov = m3_mul(m3_mul(m3_t(T), m3_t(vrk_of(cov3D))), T);
+    return {cov.c[0][0], cov.c[0][1], cov.c[1][1]};
+}
+
+// dL/dt of the lens's covariance path from dL/dJ (J = F D J_n, lens_jacobian): through J_n to the clamped mean (no
+// gradient to a clamped component) and through D's dependence on the unclamped (x, y) to t.
+__device__ __forceinline__ float3 lens_cov_dt(const LensParams& L, const LensJacobian& lj, const float dJ[2][3]) {
+    const LensPoint& p = lj.p;
+    const float3 t = lj.e.t;
+    const float iz = 1.f / t.z, iz2 = iz * iz;
+    const float a00 = L.fx * p.D00, a01 = L.fx * p.D01, a10 = L.fy * p.D01, a11 = L.fy * p.D11;
+    // dL/dJ_n = (F D)^T dL/dJ; only the entries that are not constant are needed
+    const float dn00 = a00 * dJ[0][0] + a10 * dJ[1][0];
+    const float dn02 = a00 * dJ[0][2] + a10 * dJ[1][2];
+    const float dn11 = a01 * dJ[0][1] + a11 * dJ[1][1];
+    const float dn12 = a01 * dJ[0][2] + a11 * dJ[1][2];
+    float3 dt;
+    dt.x = lj.e.x_grad_mul * -dn02 * iz2;
+    dt.y = lj.e.y_grad_mul * -dn12 * iz2;
+    dt.z = -(dn00 + dn11) * iz2 + 2.f * (t.x * dn02 + t.y * dn12) * iz2 * iz;
+    // dL/dD = F^T dL/dJ J_n^T, with D01 = D10 one variable
+    const float n02 = -t.x * iz2, n12 = -t.y * iz2;
+    const float dD00 = L.fx * (dJ[0][0] * iz + dJ[0][2] * n02);
+    const float dD01 = L.fx * (dJ[0][1] * iz + dJ[0][2] * n12) + L.fy * (dJ[1][0] * iz + dJ[1][2] * n02);
+    const float dD11 = L.fy * (dJ[1][1] * iz + dJ[1][2] * n12);
+    // dD/dx, dD/dy (d rho/dx = 2 x rho', d rho'/dx = 2 x rho'')
+    const float x = p.x, y = p.y;
+    const float dD00_dx = 6.f * x * p.drho + 4.f * x * x * x * p.ddrho + 6.f * L.p2;
+    const float pxy = 2.f * y * p.drho + 4.f * x * x * y * p.ddrho + 2.f * L.p1;   // dD00/dy = dD01/dx
+    const float qxy = 2.f * x * p.drho + 4.f * x * y * y * p.ddrho + 2.f * L.p2;   // dD01/dy = dD11/dx
+    const float dD11_dy = 6.f * y * p.drho + 4.f * y * y * y * p.ddrho + 6.f * L.p1;
+    const float gx = dD00 * dD00_dx + dD01 * pxy + dD11 * qxy;
+    const float gy = dD00 * pxy + dD01 * qxy + dD11 * dD11_dy;
+    // (x, y) = (t.x, t.y) / t.z
+    dt.x += gx * iz;
+    dt.y += gy * iz;
+    dt.z -= (gx * x + gy * y) * iz;
+    return dt;
+}
+
 // conic -> cov2D -> T and t (backward.cu:144-264): the gradients of the loss with respect to cov2D's entries a, b, c
 // (zero unless nonsingular, i.e. denom2inv != 0), to dL/d(W J)[k][j] = dL_dT[k][j] and to the clamped camera-space
 // mean t (the depth term excluded).  dL_dconic = {x, y, z} of the conic {a', b', c'}.
@@ -213,9 +318,11 @@ struct Cov2dGrad {
     float3 dL_dt;
     float aa_h;
 };
-template <bool AA = false, class Args>
+// LENS (after a lens forward): e is lj->e, and dL_dt also carries D's dependence on the mean (lens_cov_dt).
+template <bool AA = false, bool LENS = false, class Args>
 __device__ __forceinline__ Cov2dGrad cov2d_backward(const Args& a, const EwaJacobian& e, const float* cov3D,
-                                                    float3 dL_dconic, float alpha_g = 0.f) {
+                                                    float3 dL_dconic, float alpha_g = 0.f,
+                                                    const LensJacobian* lj = nullptr) {
     Cov2dGrad g;
     const float h_x = a.focal_x, h_y = a.focal_y;
     const M3& T = e.T;
@@ -261,6 +368,15 @@ __device__ __forceinline__ Cov2dGrad cov2d_backward(const Args& a, const EwaJaco
             g.dL_dT[k][j] = 2 * own * (k == 0 ? dL_da : dL_dc) + other * dL_db;
         }
     const float (&dT)[2][3] = g.dL_dT;
+    if constexpr (LENS) {
+        float dJ[2][3];
+#pragma unroll
+        for (int k = 0; k < 2; ++k)
+#pragma unroll
+            for (int i = 0; i < 3; ++i) dJ[k][i] = W.c[i][0] * dT[k][0] + W.c[i][1] * dT[k][1] + W.c[i][2] * dT[k][2];
+        g.dL_dt = lens_cov_dt(a.lens, *lj, dJ);
+        return g;
+    }
     const float dL_dJ00 = W.c[0][0] * dT[0][0] + W.c[0][1] * dT[0][1] + W.c[0][2] * dT[0][2];
     const float dL_dJ02 = W.c[2][0] * dT[0][0] + W.c[2][1] * dT[0][1] + W.c[2][2] * dT[0][2];
     const float dL_dJ11 = W.c[1][0] * dT[1][0] + W.c[1][1] * dT[1][1] + W.c[1][2] * dT[1][2];
@@ -465,24 +581,38 @@ struct Projected {
     float aa_h;   // AA: the opacity factor of the antialiasing filter
 };
 
-// Everything of forward.cu:182-237 up to (not including) the colour; false = culled.
-template <bool AA>
-__device__ __forceinline__ bool project_gaussian(const PreFwdArgs& a, const Cam& cam, int idx,
-                                                 const float3 p_orig, Projected& o) {
+// Everything of forward.cu:182-237 up to (not including) the colour; false = culled.  LENS: a: PreFwdLensArgs, the
+// mean and the covariance's Jacobian through the lens (LensParams), and the lens cull.
+template <bool AA, bool LENS = false, class Args>
+__device__ __forceinline__ bool project_gaussian(const Args& a, const Cam& cam, int idx, const float3 p_orig,
+                                                 Projected& o) {
     // near cull (auxiliary.h:152-154)
     const float3 p_view = xform4x3(p_orig, cam.view);
     if (p_view.z <= 0.2f) return false;
 
-    const float4 p_hom = xform4x4(p_orig, cam.proj);
-    const float p_w = 1.0f / (p_hom.w + 0.0000001f);
-    const float3 p_proj = {p_hom.x * p_w, p_hom.y * p_w, p_hom.z * p_w};
+    float2 point_image;
+    LensJacobian lj;
+    if constexpr (LENS) {
+        lj = lens_jacobian(a.lens, p_view, cam.view);
+        if (lj.p.s > a.lens.max_r2) return false;
+        point_image = {a.lens.fx * lj.p.xd + a.lens.cx - 0.5f, a.lens.fy * lj.p.yd + a.lens.cy - 0.5f};
+    }
+    float3 p_proj;
+    if constexpr (!LENS) {
+        const float4 p_hom = xform4x4(p_orig, cam.proj);
+        const float p_w = 1.0f / (p_hom.w + 0.0000001f);
+        p_proj = {p_hom.x * p_w, p_hom.y * p_w, p_hom.z * p_w};
+    }
 
     float cov3D[6];
     float3 scl;
     float4 rot;
     load_cov3d(a, idx, cov3D, scl, rot);
     float3 raw, cov;
-    if (AA) {
+    if constexpr (LENS) {
+        raw = cov2d_of_T(lj.e.T, cov3D);
+        cov = {raw.x + 0.3f, raw.y, raw.z + 0.3f};
+    } else if (AA) {
         raw = cov2d_ewa_raw(a, p_orig, cov3D, cam.view);
         cov = {raw.x + 0.3f, raw.y, raw.z + 0.3f};
     } else {
@@ -499,7 +629,7 @@ __device__ __forceinline__ bool project_gaussian(const PreFwdArgs& a, const Cam&
     const float lambda1 = mid + sqrtf(max(0.1f, mid * mid - det));
     const float lambda2 = mid - sqrtf(max(0.1f, mid * mid - det));
     const float my_radius = ceilf(3.f * sqrtf(max(lambda1, lambda2)));
-    const float2 point_image = {ndc_to_pix(p_proj.x, a.W), ndc_to_pix(p_proj.y, a.H)};
+    if constexpr (!LENS) point_image = {ndc_to_pix(p_proj.x, a.W), ndc_to_pix(p_proj.y, a.H)};
 
     // getRect (auxiliary.h:46-56): radius is passed as int, float division, C truncation
     const int max_radius = (int)my_radius;
@@ -517,9 +647,15 @@ __device__ __forceinline__ bool project_gaussian(const PreFwdArgs& a, const Cam&
     return true;
 }
 
-// MT = 16: SH rows of 48 floats known at compile time; 0: runtime M.  AA: the composite gets opacity * h (antialiasing)
-template <int MT, bool AA = false>
-__global__ void __launch_bounds__(PRE_THREADS) preprocess_forward_kernel(PreFwdArgs a) {
+// the lens forward's arguments: the plain ones and the lens
+struct PreFwdLensArgs : PreFwdArgs {
+    LensParams lens;
+};
+
+// MT = 16: SH rows of 48 floats known at compile time; 0: runtime M.  AA: the composite gets opacity * h (antialiasing).
+// LENS: a is a PreFwdLensArgs (preprocess_forward_lens_kernel)
+template <int MT, bool AA, bool LENS, class Args>
+__device__ __forceinline__ void preprocess_forward(const Args& a) {
     extern __shared__ float s_dyn[];
     __shared__ Cam s_cam;
     load_cam(s_cam, a.view, a.proj, a.campos);
@@ -536,7 +672,7 @@ __global__ void __launch_bounds__(PRE_THREADS) preprocess_forward_kernel(PreFwdA
         a.depth_key[idx] = DEPTH_KEY_INVISIBLE;
         a.order[idx] = (uint32_t)idx;
         p_orig = {a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2]};
-        vis = project_gaussian<AA>(a, s_cam, idx, p_orig, po);
+        vis = project_gaussian<AA, LENS>(a, s_cam, idx, p_orig, po);
     }
     uint32_t group_bit = 0;
     if (a.group) {
@@ -579,6 +715,14 @@ __global__ void __launch_bounds__(PRE_THREADS) preprocess_forward_kernel(PreFwdA
     a.rect[idx] = make_ushort4((unsigned short)po.rminx, (unsigned short)po.rminy, (unsigned short)po.rmaxx,
                                (unsigned short)po.rmaxy);
     a.tiles_touched[idx] = (po.rmaxy - po.rminy) * (po.rmaxx - po.rminx);
+}
+template <int MT, bool AA = false>
+__global__ void __launch_bounds__(PRE_THREADS) preprocess_forward_kernel(PreFwdArgs a) {
+    preprocess_forward<MT, AA, false>(a);
+}
+template <int MT, bool AA>
+__global__ void __launch_bounds__(PRE_THREADS) preprocess_forward_lens_kernel(PreFwdLensArgs a) {
+    preprocess_forward<MT, AA, true>(a);
 }
 
 // rasterizer_impl.cu:54-66
@@ -653,12 +797,17 @@ __device__ __forceinline__ float3 dnormvdv3(float3 v, float3 dv) {   // auxiliar
     return r;
 }
 
-// Register budget capped for 8 resident blocks per SM (64 registers, 20 spilled words): the kernel is HBM-bound and
-// gains from more loads in flight than the unconstrained 96 registers allow.
+// the lens backward's arguments: the plain ones and the lens of the forward
+struct PreBwdLensArgs : PreBwdArgs {
+    LensParams lens;
+};
+
 // MT = 16: compile-time SH row length; 0: runtime M.  DP: gradients go to a.sink.  AA: after an antialiased forward.
-template <int MT, bool DP = false, bool AA = false>
-__global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(const __grid_constant__ PreBwdArgs a) {
+// LENS: after a lens forward, a is a PreBwdLensArgs (preprocess_backward_lens_kernel).
+template <int MT, bool DP, bool AA, bool LENS, class Args>
+__device__ __forceinline__ void preprocess_backward(const Args& a) {
     static_assert(!(DP && AA), "the fused gradient exchange does not take the antialiased backward");
+    static_assert(!(DP && LENS), "the fused gradient exchange does not take the lens backward");
     extern __shared__ float s_dyn[];
     __shared__ Cam s_cam;
     load_cam(s_cam, a.view, a.proj, a.campos);
@@ -733,11 +882,15 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(con
         float3 scl;
         float4 rot;
         load_cov3d(a, idx, cov3D, scl, rot);
+        LensJacobian lj;
+        if constexpr (LENS) lj = lens_jacobian(a.lens, xform4x3(mean, view), view);
         // ---- conic -> cov2D -> cov3D, mean (backward.cu:144-274) ----------
         {
-            const EwaJacobian e = ewa_jacobian(a, mean, view);
-            const Cov2dGrad cg = cov2d_backward<AA>(a, e, cov3D, make_float3(g[2], g[3], g[4]),
-                                                    AA ? a.Cod[idx].y * g[5] : 0.f);
+            EwaJacobian e;
+            if constexpr (LENS) e = lj.e;
+            else e = ewa_jacobian(a, mean, view);
+            const Cov2dGrad cg = cov2d_backward<AA, LENS>(a, e, cov3D, make_float3(g[2], g[3], g[4]),
+                                                          AA ? a.Cod[idx].y * g[5] : 0.f, &lj);
             if (AA) aa_h = cg.aa_h;
             if (cg.nonsingular) {
                 const M3& T = e.T;
@@ -765,7 +918,24 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(con
             dmean[2] = view[8] * dt.x + view[9] * dt.y + view[10] * dt.z;
         }
         // ---- screen-space mean and depth terms (backward.cu:372-403) ------
-        {
+        if constexpr (LENS) {
+            // pixel = F (xd, yd) + c - 0.5: dL/d(x, y) = D^T F dL/dpixel, then (x, y) = (t.x, t.y) / t.z
+            const LensParams& L = a.lens;
+            const LensPoint& p = lj.p;
+            const float gxd = L.fx * L.ndc_x * g[0], gyd = L.fy * L.ndc_y * g[1];
+            const float gx = p.D00 * gxd + p.D01 * gyd, gy = p.D01 * gxd + p.D11 * gyd;
+            const float iz = 1.f / lj.e.t.z;
+            const float3 dt = {gx * iz, gy * iz, -(gx * p.x + gy * p.y) * iz};
+            dmean[0] += view[0] * dt.x + view[1] * dt.y + view[2] * dt.z;
+            dmean[1] += view[4] * dt.x + view[5] * dt.y + view[6] * dt.z;
+            dmean[2] += view[8] * dt.x + view[9] * dt.y + view[10] * dt.z;
+            const float3 m = mean;
+            const float mul3 = view[2] * m.x + view[6] * m.y + view[10] * m.z + view[14];
+            const float gd = g[9];
+            dmean[0] += (view[2] - view[3] * mul3) * gd;
+            dmean[1] += (view[6] - view[7] * mul3) * gd;
+            dmean[2] += (view[10] - view[11] * mul3) * gd;
+        } else {
             const float3 m = mean;
             const float4 m_hom = xform4x4(m, proj);
             const float m_w = 1.0f / (m_hom.w + 0.0000001f);
@@ -907,6 +1077,17 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(con
     a.dL_dscale[3 * idx + 1] = dscale[1];
     a.dL_dscale[3 * idx + 2] = dscale[2];
     reinterpret_cast<float4*>(a.dL_drot)[idx] = make_float4(drot[0], drot[1], drot[2], drot[3]);
+}
+// Register budget capped for 8 resident blocks per SM (64 registers, 20 spilled words): the kernel is HBM-bound and
+// gains from more loads in flight than the unconstrained 96 registers allow.
+template <int MT, bool DP = false, bool AA = false>
+__global__ void __launch_bounds__(PRE_THREADS, 8) preprocess_backward_kernel(const __grid_constant__ PreBwdArgs a) {
+    preprocess_backward<MT, DP, AA, false>(a);
+}
+template <int MT, bool AA>
+__global__ void __launch_bounds__(PRE_THREADS, 8)
+preprocess_backward_lens_kernel(const __grid_constant__ PreBwdLensArgs a) {
+    preprocess_backward<MT, false, AA, true>(a);
 }
 
 }  // namespace s3g

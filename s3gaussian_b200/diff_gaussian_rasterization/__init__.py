@@ -139,6 +139,37 @@ def _camera_inputs(raster_settings):
     return None
 
 
+class Lens(NamedTuple):
+    """A camera's intrinsics and OpenCV radial-tangential distortion, in pixels of the render size (s3g_raster_lens,
+    include/s3g_b200.h).  Pixel j's centre is at j + 0.5, so a centred camera has cx = width / 2; an OpenCV K, whose
+    pixel centres are at j, needs cx + 0.5 and cy + 0.5."""
+    fx: float
+    fy: float
+    cx: float
+    cy: float
+    k1: float = 0.0
+    k2: float = 0.0
+    p1: float = 0.0
+    p2: float = 0.0
+    k3: float = 0.0
+
+
+def _lens_struct(lens):
+    return _lib.RasterLens(*(float(v) for v in lens))
+
+
+def _lens_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
+                colors_aux, opacity, antialiasing, absgrad, lens):
+    """_RasterizeGaussians.apply of a lens forward: every input given, the lens last.  Camera gradients do not pass
+    through the lens."""
+    if _camera_inputs(raster_settings) is not None:
+        raise NotImplementedError("camera gradients through a lens are not implemented: detach viewmatrix, projmatrix "
+                                  "and campos, or render without the lens")
+    return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                     cov3Ds_precomp, raster_settings, colors_aux, None, None, None, opacity,
+                                     bool(antialiasing), bool(absgrad), Lens(*lens))
+
+
 def _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                        raster_settings, colors_aux, opacity, antialiasing=True, absgrad=False):
     """_RasterizeGaussians.apply of an antialiased or absgrad forward: every optional input given, then the opacity
@@ -151,7 +182,10 @@ def _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, 
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                        cov3Ds_precomp, raster_settings, antialiasing=False, absgrad=False):
+                        cov3Ds_precomp, raster_settings, antialiasing=False, absgrad=False, lens=None):
+    if lens is not None:
+        return _lens_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                           raster_settings, None, False, antialiasing, absgrad, lens)
     if antialiasing or absgrad:
         return _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                   cov3Ds_precomp, raster_settings, None, False, antialiasing, absgrad)
@@ -164,9 +198,12 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales,
 
 
 def rasterize_gaussians_aux(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                            cov3Ds_precomp, raster_settings, colors_aux, antialiasing=False, absgrad=False):
+                            cov3Ds_precomp, raster_settings, colors_aux, antialiasing=False, absgrad=False, lens=None):
     """(color, radii, depth, color_aux): both colour sets composited on ONE preprocess + sort
     (the aux pair of s3g_rasterize_forward / s3g_rasterize_backward)."""
+    if lens is not None:
+        return _lens_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                           raster_settings, colors_aux, False, antialiasing, absgrad, lens)
     if antialiasing or absgrad:
         return _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                   cov3Ds_precomp, raster_settings, colors_aux, False, antialiasing, absgrad)
@@ -179,9 +216,13 @@ def rasterize_gaussians_aux(means3D, means2D, sh, colors_precomp, opacities, sca
 
 
 def rasterize_gaussians_opacity(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                cov3Ds_precomp, raster_settings, colors_aux=None, antialiasing=False, absgrad=False):
+                                cov3Ds_precomp, raster_settings, colors_aux=None, antialiasing=False, absgrad=False,
+                                lens=None):
     """(color, radii, depth, alpha, median_depth[, color_aux]): the opacity images of s3g_rasterize_forward_opacity
     from the same walk, differentiable like the others (the *_opacity backwards)."""
+    if lens is not None:
+        return _lens_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                           raster_settings, colors_aux, True, antialiasing, absgrad, lens)
     if antialiasing or absgrad:
         return _antialiased_apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                   cov3Ds_precomp, raster_settings, colors_aux, True, antialiasing, absgrad)
@@ -234,7 +275,8 @@ def _forward_args(means3D, sh, colors_precomp, opacities, scales, rotations, cov
 
 
 def rasterize_gaussians_eval(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                             raster_settings, group=None, flow_colors=(), with_opacity=False, antialiasing=False):
+                             raster_settings, group=None, flow_colors=(), with_opacity=False, antialiasing=False,
+                             lens=None):
     """s3g_rasterize_forward with its forward-only extras: (color, radii, depth, decomposition, flows) from one
     preprocess, one sort and one composite walk.  decomposition is (color_d, depth_d, color_s, depth_s) when
     `group` (bool or uint8 [P] on the device) is given, else None: the images forward() gives for the Gaussians
@@ -242,8 +284,9 @@ def rasterize_gaussians_eval(means3D, means2D, sh, colors_precomp, opacities, sc
     `flow_colors` (at most two float32 [P,4] device tensors, rgb in [:, :3], as s3g_flow_colors writes them), each
     the image forward() gives with colors_precomp = that rgb.  with_opacity adds a sixth element, (alpha,
     median_depth, alpha_d, alpha_s) as forward_opacity() defines them; alpha_d / alpha_s are the dynamic and static
-    subsets' alpha images, None without `group`.  antialiasing: s3g_rasterize_forward_antialiased instead.  Forward
-    only: there is no autograd node."""
+    subsets' alpha images, None without `group`.  antialiasing: s3g_rasterize_forward_antialiased instead.  lens (a
+    Lens): s3g_rasterize_forward_lens, through the camera's intrinsics and distortion.  Forward only: there is no
+    autograd node."""
     lib = _lib.load()
     flow_colors = tuple(flow_colors)
     if len(flow_colors) > 2:
@@ -271,6 +314,17 @@ def rasterize_gaussians_eval(means3D, means2D, sh, colors_precomp, opacities, sc
     for k, (fc, out) in enumerate(zip(flow_colors, flows)):
         fwd.flow_colors[k], fwd.out_flow[k] = _ptr(fc), out.data_ptr()
     with torch.cuda.device(dev):
+        if lens is not None:
+            opacity = None
+            if with_opacity:
+                opacity = tuple(torch.empty_like(depth) if i < 2 or group is not None else None for i in range(4))
+                opa = _lib.RasterOpacityArgs(*(_ptr(t) for t in opacity))
+            lens_s = _lens_struct(lens)
+            _lib.check(lib.s3g_rasterize_forward_lens(C.byref(scene), C.byref(fwd), C.byref(opa) if with_opacity
+                                                      else None, 1 if antialiasing else 0, C.byref(lens_s),
+                                                      _stream_ptr(dev)), "rasterize_gaussians_eval")
+            out = (color, radii, depth, decomposition, flows)
+            return out + (opacity,) if with_opacity else out
         if not with_opacity:
             if antialiasing:
                 _lib.check(lib.s3g_rasterize_forward_antialiased(C.byref(scene), C.byref(fwd), None,
@@ -362,12 +416,13 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                 cov3Ds_precomp, raster_settings, colors_aux=None, viewmatrix=None, projmatrix=None, campos=None,
-                opacity=False, antialiasing=False, absgrad=False):
+                opacity=False, antialiasing=False, absgrad=False, lens=None):
         # viewmatrix / projmatrix / campos: raster_settings' own tensors, passed (by rasterize_gaussians*) only when
         # one of them requires grad; the backward then returns their gradients.  opacity (rasterize_gaussians_opacity):
         # alpha and median_depth follow depth in the outputs.  antialiasing: s3g_rasterize_forward_antialiased, whose
         # chain rule the backward calls apply by themselves.  absgrad: the backward is s3g_rasterize_backward_absgrad
-        # and sets (or adds to) the `absgrad` attribute of the tensor object passed as means2D
+        # and sets (or adds to) the `absgrad` attribute of the tensor object passed as means2D.  lens (a Lens):
+        # s3g_rasterize_forward_lens, whose chain rule the backward calls apply by themselves
         lib = _lib.load()
         rs = raster_settings
         scene, fwd, lease, inputs, color, depth, radii = _forward_args(means3D, sh, colors_precomp, opacities, scales,
@@ -384,7 +439,14 @@ class _RasterizeGaussians(torch.autograd.Function):
         if opacity:
             alpha, median_depth = torch.empty_like(depth), torch.empty_like(depth)
             opa = _lib.RasterOpacityArgs(out_alpha=alpha.data_ptr(), out_median_depth=median_depth.data_ptr())
-        if antialiasing:
+        if lens is not None:
+            if viewmatrix is not None:
+                raise NotImplementedError("camera gradients through a lens are not implemented")
+            lens_s = _lens_struct(lens)
+            forward_call = lambda: lib.s3g_rasterize_forward_lens(
+                C.byref(scene), C.byref(fwd), C.byref(opa) if opacity else None, 1 if antialiasing else 0,
+                C.byref(lens_s), _stream_ptr(dev))
+        elif antialiasing:
             forward_call = lambda: lib.s3g_rasterize_forward_antialiased(
                 C.byref(scene), C.byref(fwd), C.byref(opa) if opacity else None, _stream_ptr(dev))
         elif opacity:
@@ -425,6 +487,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.opacity = bool(opacity)
         ctx.antialiasing = bool(antialiasing)
         ctx.absgrad = bool(absgrad)
+        ctx.lens = lens is not None
         if absgrad:
             ctx.means2D = means2D
         out = (color, radii, depth) + ((alpha, median_depth) if opacity else ()) + ((color_aux,) if has_aux else ())
@@ -436,6 +499,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         opacity = getattr(ctx, "opacity", False)
         antialiasing = getattr(ctx, "antialiasing", False)
         absgrad = getattr(ctx, "absgrad", False)
+        lens = getattr(ctx, "lens", False)
         grad_alpha, grad_median = grad_rest[:2] if opacity else (None, None)
         grad_rest = grad_rest[2:] if opacity else grad_rest
         grad_out_aux = grad_rest[0] if grad_rest else None
@@ -507,6 +571,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                 raise NotImplementedError("FusedGradExchange: precomputed 3-D covariances are not exchanged")
             if antialiasing:
                 raise NotImplementedError("FusedGradExchange: an antialiased forward's gradients are not exchanged")
+            if lens:
+                raise NotImplementedError("FusedGradExchange: a lens forward's gradients are not exchanged")
             _GRAD_SINK.note_backward()
             bwd.sink = C.pointer(peer)
         # the kernel stores dL_drot 16 bytes per row: a sink's view off a 16-byte boundary (a flat bucket holding the
@@ -553,6 +619,8 @@ class _RasterizeGaussians(torch.autograd.Function):
             m2 = ctx.means2D
             prev = getattr(m2, "absgrad", None)
             m2.absgrad = grad_abs if prev is None else prev + grad_abs
+        if lens:   # every input was given (_lens_apply)
+            return grads + (grad_aux, None, None, None, None, None, None, None)
         if ctx.has_aux:
             grads = grads + (grad_aux,)
         if ctx.camera or opacity or antialiasing or absgrad:
@@ -608,13 +676,20 @@ class GaussianRasterizer(nn.Module):
     component, in the units of means2D.grad, and store it as `means2D.absgrad` (float32 [P,2], zero for Gaussians
     with radii <= 0) on the tensor object passed as means2D.  A second backward into the same object adds to it, as
     .grad accumulates; set it to None to start again.  The statistic is per call: the aux pair's two images share one
-    sum, two separate calls add two.  Not in the reference."""
+    sum, two separate calls add two.  Not in the reference.
 
-    def __init__(self, raster_settings, antialiasing=False, absgrad=False):
+    lens (a Lens, or anything unpacking to fx, fy, cx, cy[, k1, k2, p1, p2, k3]): every forward projects through the
+    camera's own intrinsics and OpenCV radial-tangential distortion (s3g_rasterize_forward_lens, include/s3g_b200.h)
+    instead of the centred pinhole of tanfovx / tanfovy; viewmatrix still places the camera.  The backwards
+    differentiate that projection; the lens gets no gradient, and camera gradients through it are not implemented
+    (NotImplementedError when viewmatrix, projmatrix or campos requires grad).  Not in the reference."""
+
+    def __init__(self, raster_settings, antialiasing=False, absgrad=False, lens=None):
         super().__init__()
         self.raster_settings = raster_settings
         self.antialiasing = bool(antialiasing)
         self.absgrad = bool(absgrad)
+        self.lens = None if lens is None else Lens(*lens)
 
     def markVisible(self, positions):
         """bool[P]: passes the near-plane test (rasterizer_impl.cu:54-66)."""
@@ -638,7 +713,8 @@ class GaussianRasterizer(nn.Module):
         shs, colors_precomp, scales, rotations, cov3D_precomp = _reference_inputs(shs, colors_precomp, scales,
                                                                                   rotations, cov3D_precomp)
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales,
-                                   rotations, cov3D_precomp, self.raster_settings, self.antialiasing, self.absgrad)
+                                   rotations, cov3D_precomp, self.raster_settings, self.antialiasing, self.absgrad,
+                                   self.lens)
 
     def forward_aux(self, means3D, means2D, opacities, colors_aux, shs=None, colors_precomp=None, scales=None,
                     rotations=None, cov3D_precomp=None):
@@ -649,7 +725,7 @@ class GaussianRasterizer(nn.Module):
                                                                                   rotations, cov3D_precomp)
         return rasterize_gaussians_aux(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                        cov3D_precomp, self.raster_settings, colors_aux, self.antialiasing,
-                                       self.absgrad)
+                                       self.absgrad, self.lens)
 
     def forward_opacity(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                         cov3D_precomp=None, colors_aux=None):
@@ -663,7 +739,7 @@ class GaussianRasterizer(nn.Module):
                                                                                   rotations, cov3D_precomp)
         return rasterize_gaussians_opacity(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                            cov3D_precomp, self.raster_settings, colors_aux, self.antialiasing,
-                                           self.absgrad)
+                                           self.absgrad, self.lens)
 
     def forward_eval(self, means3D, means2D, opacities, group=None, flow_colors=(), shs=None, colors_precomp=None,
                      scales=None, rotations=None, cov3D_precomp=None, with_opacity=False):
@@ -681,4 +757,4 @@ class GaussianRasterizer(nn.Module):
                                                                                   rotations, cov3D_precomp)
         return rasterize_gaussians_eval(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                         cov3D_precomp, self.raster_settings, group, flow_colors, with_opacity,
-                                        self.antialiasing)
+                                        self.antialiasing, self.lens)

@@ -172,7 +172,8 @@ def render_pixels(viewpoint_stack, gaussians, bg, pipe, compute_metrics: bool = 
     (sky.sky_camera gives its c2w / intrinsic); the alpha image comes from the same walk.  The static / dynamic
     images are unchanged.
     """
-    from .gaussian_renderer import dynamic_mask_of, fine_front, pipe_rasterizer_kwargs, raster_settings_for
+    from .gaussian_renderer import (dynamic_mask_of, fine_front, pipe_lens_kwargs, pipe_rasterizer_kwargs,
+                                    raster_settings_for)
     from .diff_gaussian_rasterization import GaussianRasterizer
     rgbs, gt_rgbs, depths, static_rgbs, dynamic_rgbs = [], [], [], [], []
     opacities, median_depths, static_opacities, dynamic_opacities = [], [], [], []
@@ -210,7 +211,8 @@ def render_pixels(viewpoint_stack, gaussians, bg, pipe, compute_metrics: bool = 
                 if a not in colours:
                     colours[a] = flow_colors(dx_list[a + NUM_CAMS], dx_list[a], normalize=debug)
             group = dynamic_mask_of(dx) if return_decomposition and dx is not None else None
-            out = GaussianRasterizer(raster_settings=rs, **pipe_rasterizer_kwargs(pipe)).forward_eval(
+            out = GaussianRasterizer(raster_settings=rs, **pipe_rasterizer_kwargs(pipe),
+                                     **pipe_lens_kwargs(pipe, cam)).forward_eval(
                 means3D=means3D, means2D=torch.zeros_like(means3D), opacities=opacity, group=group,
                 flow_colors=[colours[a] for a in need], shs=shs, colors_precomp=colors_precomp, scales=scales,
                 rotations=rotations, **({"with_opacity": True} if with_opacity or sky_model is not None else {}))

@@ -79,6 +79,7 @@ class PipelineParams:       # arguments/__init__.py:93-98 defaults
     antialiasing = False    # ours: the rasterizer's antialiasing filter (GaussianRasterizer(antialiasing=True))
     filter_3d = False       # ours: Mip-Splatting's 3-D smoothing filter on the scales and opacities (pc.filter_3D)
     absgrad = False         # ours: the backward also sets viewspace_points.absgrad (GaussianRasterizer(absgrad=True))
+    lens = False            # ours: project through the camera's intrinsic and distortion (GaussianRasterizer(lens=...))
 
 
 def pipe_shared_binning(pipe) -> bool:
@@ -96,6 +97,26 @@ def pipe_rasterizer_kwargs(pipe) -> dict:
     if getattr(pipe, "absgrad", False):
         kw["absgrad"] = True
     return kw
+
+
+def camera_lens(viewpoint_camera):
+    """The Lens of a camera: fx, fy, cx, cy from its 3x3 `intrinsic` (the reference's Camera.intrinsic, principal point
+    with pixel centres at j + 0.5) and k1, k2, p1, p2, k3 from its `distortion` (zeros when it has none)."""
+    from .diff_gaussian_rasterization import Lens
+    K = getattr(viewpoint_camera, "intrinsic", None)
+    if K is None:
+        raise RuntimeError("pipe.lens: the camera has no intrinsic (3x3 K) to build the lens from")
+    K = torch.as_tensor(K, dtype=torch.float64).reshape(3, 3).cpu()
+    dist = getattr(viewpoint_camera, "distortion", None)
+    dist = [0.0] * 5 if dist is None else [float(v) for v in torch.as_tensor(dist, dtype=torch.float64).reshape(-1)]
+    if len(dist) != 5:
+        raise RuntimeError(f"pipe.lens: camera.distortion must hold k1, k2, p1, p2, k3 ({len(dist)} values)")
+    return Lens(float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), *dist)
+
+
+def pipe_lens_kwargs(pipe, viewpoint_camera) -> dict:
+    """{"lens": camera_lens(viewpoint_camera)} when pipe.lens is set, else nothing."""
+    return {"lens": camera_lens(viewpoint_camera)} if getattr(pipe, "lens", False) else {}
 
 
 def pipe_filter_3d(pipe, pc) -> bool:
@@ -118,6 +139,7 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
            stage="fine", return_decomposition=False, return_dx=False, render_feat=False):
     """Render the scene.  Background tensor (bg_color) must be on GPU!
 
+    With pipe.lens, every rasterizer call projects through the camera's `intrinsic` and `distortion` (camera_lens).
     With pipe.absgrad, the backward of the result also sets result["viewspace_points"].absgrad (float32 [P,2]), the
     absolute screen-space gradient of the call(s) that drew "render" and "feat" (GaussianRasterizer(absgrad=True)).
     The differentiable decomposition passes index means2D and leave their statistic on those temporaries."""
@@ -133,7 +155,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
 
     raster_settings = raster_settings_for(viewpoint_camera, pc, pipe, bg_color, scaling_modifier)
     campos = raster_settings.campos
-    rasterizer = GaussianRasterizer(raster_settings=raster_settings, **pipe_rasterizer_kwargs(pipe))
+    rasterizer = GaussianRasterizer(raster_settings=raster_settings, **pipe_rasterizer_kwargs(pipe),
+                                    **pipe_lens_kwargs(pipe, viewpoint_camera))
 
     means2D = screenspace_points
     shs = pc.get_features

@@ -186,8 +186,9 @@ class Background_Model(nn.Module):   # noqa: N801 (the reference's name)
 
 def sky_camera(viewpoint_cam):
     """``(c2w [4,4], intrinsic [3,3])`` float32 of a camera: a reference camera's own ``c2w`` / ``intrinsic``
-    (scene/cameras.py) when it has them; otherwise derived from ``world_view_transform`` (W2C transposed) and the
-    fields of view, with the principal point at the image centre (``SyntheticCamera``).  With that intrinsic, the sky
+    (scene/cameras.py) when it has them; otherwise ``c2w`` derived from ``world_view_transform`` (W2C transposed) and
+    the camera's own ``intrinsic`` when it has one, else one from the fields of view with the principal point at the
+    image centre (``SyntheticCamera``).  With that intrinsic, the sky
     direction of pixel (x, y) projects through ``full_proj_transform`` onto the rasterizer's centre of that pixel."""
     c2w = getattr(viewpoint_cam, "c2w", None)
     K = getattr(viewpoint_cam, "intrinsic", None)
@@ -196,6 +197,8 @@ def sky_camera(viewpoint_cam):
         return c2w.to(torch.float32).reshape(4, 4).contiguous(), K.to(torch.float32).reshape(3, 3).contiguous()
     wvt = viewpoint_cam.world_view_transform
     c2w = torch.linalg.inv(wvt.transpose(0, 1).double()).to(torch.float32).contiguous()
+    if K is not None:
+        return c2w, torch.as_tensor(K).to(device=c2w.device, dtype=torch.float32).reshape(3, 3).contiguous()
     W, H = viewpoint_cam.image_width, viewpoint_cam.image_height
     fx = W / (2.0 * math.tan(viewpoint_cam.FoVx * 0.5))
     fy = H / (2.0 * math.tan(viewpoint_cam.FoVy * 0.5))

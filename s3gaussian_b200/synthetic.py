@@ -46,12 +46,15 @@ class SyntheticCamera:
     full_proj_transform: torch.Tensor    # [4,4]
     camera_center: torch.Tensor          # [3]
     time: float = 0.0
+    # optional, for render(pipe.lens): the 3x3 K (pixel centres at j + 0.5) and OpenCV k1, k2, p1, p2, k3
+    intrinsic: torch.Tensor | None = None
+    distortion: torch.Tensor | None = None
 
     def to(self, device):
         return SyntheticCamera(self.image_width, self.image_height, self.FoVx, self.FoVy,
                                self.world_view_transform.to(device),
                                self.full_proj_transform.to(device), self.camera_center.to(device),
-                               self.time)
+                               self.time, self.intrinsic, self.distortion)
 
     @property
     def tanfovx(self):
